@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- benchmarks of the native GridLLM worker on B200 (BASELINE.json configs 2-5; config 2 is the headline default).
+"""bench.py -- benchmarks of the native GridLLM worker on H100 (BASELINE.json configs 2-5; config 2 is the headline default).
 
   --workload config2 (default)  Llama-3-8B q4_K_M, greedy, 512-in / 128-out, batch 1 per GPU           generated tokens/s
   --workload config3            the same model, 32 concurrent streamed chat requests per GPU (256 on 8)   generated tokens/s
@@ -19,6 +19,10 @@ config4: 32 x 2048 prompt tokens; config5: 1 250 documents / 8 = the share of on
 measured bounded sample -- and prints the same metric / unit / config as the native arm.  (The reference's own engine, an
 un-vendored Ollama/llama.cpp behind HTTP, cannot be installed here: no node / ollama / network -- DESIGN.md section 2.)
 
+--dump-outputs DIR writes what the timed path returned in its last step (config2: generated ids and logprobs; config3: the
+streamed responses as bytes; config4: the next-token id and logprob of each sequence; config5: the embeddings) as DIR/<name>.npy
+in float32 / float64.  Inputs are seeded: two builds given the same arguments can be compared output for output.
+
 Launch: python bench.py [--gpus N --steps K --warmup W]; N>1 via torchrun (one rank per GPU, no data-path collective: requests
 are independent, SURVEY.md section 8e) -- weak scaling.  `--workload config3 --gpus N` WITHOUT torchrun runs N engines in ONE
 process behind one scheduler (the north_star's in-process shape).
@@ -33,6 +37,7 @@ import os
 import statistics
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -86,7 +91,7 @@ def build_model_once(key: str, rank: int, barrier) -> str:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, device: int):
         self.device = device
@@ -146,13 +151,13 @@ def physical_cores() -> int:
 
 
 class CpuRestatement:
-    """oracle/c/llama_cpu.c on this box's host cores.  Prefers a -march=native build made here (oracle/_ref is git-ignored and
-    travels to the GPU box); falls back to the portable prebuilt library."""
+    """oracle/c/llama_cpu.c on the host cores.  Prefers a -march=native build made at run time in the temporary directory (the
+    tree may be read-only); falls back to the portable library build() made."""
 
     def __init__(self, path: str, n_ctx: int):
         src = os.path.join(ROOT, "oracle", "c", "llama_cpu.c")
         so = os.path.join(ROOT, "oracle", "_ref", "liboracle_cpu.so")
-        native = os.path.join(ROOT, "oracle", "_ref", f"liboracle_cpu_native_{os.getuid()}.so")
+        native = native_cpu_lib_path()
         lib = None
         try:
             cc = "/usr/bin/gcc" if os.path.exists("/usr/bin/gcc") else "gcc"
@@ -234,6 +239,10 @@ class CpuRestatement:
         self.lib.oc_free(self.h)
 
 
+def native_cpu_lib_path() -> str:
+    return os.path.join(tempfile.gettempdir(), f"gridllm_oracle_cpu_native_{os.getuid()}.so")
+
+
 def cpu_step(cpu: CpuRestatement, workload: str, seed: int):
     """one bounded CPU sample of `workload` -> (units produced, seconds, description)"""
     if workload in ("config2", "config3"):
@@ -260,6 +269,7 @@ def main():
     ap.add_argument("--batch", type=int, default=32, help="config3: concurrent requests per GPU")
     ap.add_argument("--docs", type=int, default=1250, help="config5: documents per GPU per step (10 000 / 8 workers)")
     ap.add_argument("--batch-weights", type=int, default=0, help="config3: 0 auto, 1 resident 16-bit weights, 2 quantised weights")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     wl = args.workload
     # a stall must leave evidence: every thread's stack goes to stderr if the run makes no visible progress for a while
@@ -305,7 +315,7 @@ def main():
         "config5": {"workload": f"Mistral-7B q8_0 synthetic GGUF, embeddings of {DOC_TOKENS}-token documents, {args.docs} documents per GPU per step "
                                 "(10 000 over 8 workers: BASELINE.json configs[4])", "docs_per_gpu_per_step": args.docs, "doc_tokens": DOC_TOKENS},
     }[wl]
-    config["l2_policy"] = "weights (4.9-16 GB per pass) >> 126 MB L2: inputs larger than L2"
+    config["l2_policy"] = "weights (4.9-16 GB per pass) >> 50 MB L2: inputs larger than L2"
     config["parallelism"] = f"replicas x{n_gpus} (request sharding, no collective)"
 
     # ---------------------------------------------------------------- reference arm (CPU restatement, really timed)
@@ -341,10 +351,10 @@ def main():
         raise SystemExit("bench.py: no CUDA device for this rank -- the native worker has no CPU fallback")
     torch.cuda.set_device(local_rank)
     path = build_model_once(mkey, rank, barrier)
-    peaks = {"hbm_gbs": 6650.0, "tf": 1464.2, "src": "fallback (B200_PROFILING.md)"}
+    peaks = {"hbm_gbs": 3350.0, "tf": 989.4, "src": "H100 SXM data sheet (3.35 TB/s HBM3, 989 dense fp16 / bf16 TFLOP/s at 700 W)"}
     try:
         pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        peaks = {"hbm_gbs": float(pk["hbm_gbs"]), "tf": float(pk.get("bf16_tflops_sustained", 1464.2)), "src": "measured (MEASURED_PEAKS.json)"}
+        peaks = {"hbm_gbs": float(pk["hbm_gbs"]), "tf": float(pk.get("bf16_tflops_sustained", 989.4)), "src": "measured (MEASURED_PEAKS.json)"}
     except Exception:
         pass
     sampler = ClockSampler(local_rank)
@@ -375,6 +385,8 @@ def main():
                 "data": "synthetic", "config": config, "e2e": out["e2e"], "gpu_launches": out["gpu_launches"], "roofline": out["roofline"],
                 "clocks": out["clocks"]}
         line.update(out.get("extra", {}))
+        if args.dump_outputs:
+            line["dumped_outputs"] = dump_outputs(args.dump_outputs, out["dump"])
         if not args.no_cpu and world == 1:                # the contract: the cpu_baseline leg on rank 0 at N = 1 only
             # the CPU leg runs in its own process (the reference arm of this same file, two measured samples after a warm one): the
             # engines are gone by now, and an OpenMP runtime started inside a process that has run CUDA, asyncio and a batch-runner
@@ -393,6 +405,31 @@ def main():
         dist.destroy_process_group()
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(d: str, arrays: dict) -> dict:
+    """arrays (name -> numpy array) -> d/<name>.npy, integers as float64 and floats as float32.  A larger total than
+    DUMP_LIMIT_BYTES keeps, of the largest arrays, one fixed, seeded sample of rows each, drawn once from the full output;
+    <name>_sample_rows holds the indices of the kept rows in that output."""
+    os.makedirs(d, exist_ok=True)
+    out = {k: np.asarray(v).astype(np.float32 if np.asarray(v).dtype.kind == "f" else np.float64) for k, v in arrays.items()}
+    sampled = set()
+    while sum(a.nbytes for a in out.values()) > DUMP_LIMIT_BYTES:
+        k = max((n for n in out if n not in sampled and not n.endswith("_sample_rows")), key=lambda n: out[n].nbytes)
+        a = out[k]
+        row_bytes = a.nbytes // a.shape[0] + 8                      # the kept row and its index
+        budget = DUMP_LIMIT_BYTES - sum(b.nbytes for n, b in out.items() if n != k)
+        keep = int(min(a.shape[0], max(1, budget // row_bytes)))
+        rows = np.sort(np.random.Generator(np.random.PCG64(0)).choice(a.shape[0], size=keep, replace=False))
+        out[k] = a[rows]
+        out[k + "_sample_rows"] = rows.astype(np.float64)
+        sampled.add(k)
+    for k, a in out.items():
+        np.save(os.path.join(d, k + ".npy"), a)
+    return {k: list(a.shape) for k, a in out.items()}
+
+
 def prompt_for(i: int, n: int = N_PROMPT, vocab: int = 128000) -> np.ndarray:
     return np.random.Generator(np.random.PCG64(1000 + i)).integers(0, vocab, size=n).astype(np.int32)
 
@@ -403,7 +440,7 @@ def preflight_8b_parity(eng, path: str) -> dict:
     tokens + 4 greedy tokens through the decode kernels at the full Llama-3-8B shape (32 layers, 128 256-entry vocabulary, K = 14336
     in 4 K-segments, GQA 4:1).  Tolerances of tests/test_gpu_decode.py: logits within 1e-2 * max|logit| of exact arithmetic, logprob
     within 2e-2, ids equal wherever the oracle's top-1/top-2 margin exceeds 5e-2.  Raises on a mismatch: a fast wrong kernel is not a result."""
-    so = os.path.join(ROOT, "oracle", "_ref", f"liboracle_cpu_native_{os.getuid()}.so")
+    so = native_cpu_lib_path()
     if not os.path.exists(so):
         so = os.path.join(ROOT, "oracle", "_ref", "liboracle_cpu.so")
     lib = C.CDLL(so)
@@ -491,12 +528,12 @@ def run_config2(args, N, path, rank, local_rank, world, dist, timed, peaks, extr
             "roofline": {"bound": "hbm", "kernel": "gemv_kernel (all weight GEMVs of one decode step, ctx 576)", "achieved": achieved, "peak": peaks["hbm_gbs"],
                          "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"], "peak_source": peaks["src"], "algorithmic_bytes_per_token": bpt,
                          "ms_per_decode_step": ms_tok, "launches_per_decode_step": nl_tok,
-                         "traffic": None, "traffic_note": "DRAM bytes == algorithmic bytes to 0.02 % in the committed ncu --set full capture "
-                                                          "(profiles/r01_run59_ncu_summary.md); not re-measured by this run"},
+                         "traffic": None, "traffic_note": "DRAM traffic not measured by this run"},
             "clocks": clocks,
             "extra": {"breakdown": {"prefill_ms_per_request": prefill_ns / args.steps * 1e-6, "decode_ms_per_request": (dev_ns - prefill_ns) / args.steps * 1e-6,
                                     "decode_tok_s_per_gpu": N_GEN / ((dev_ns - prefill_ns) / args.steps * 1e-9)},
-                      "parity_preflight": pre}}
+                      "parity_preflight": pre},
+            "dump": {"ids": last.ids, "logprobs": last.logprobs}}
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -557,7 +594,11 @@ def run_config3(args, N, path, rank, local_rank, world, dist, timed, peaks, extr
         chunks = sum(sched.stream_chunks.get(j["id"], 0) for j in jobs)
         used = sorted(set(sched.assigned.values()))
         ttft = [sched.first_chunk_at[j["id"]] - sched.submitted_at[j["id"]] for j in jobs if j["id"] in sched.first_chunk_at]
-        return {"wall": wall, "ok": ok, "chunks": chunks, "workers_used": used, "ticks": sched.ticks, "n": len(jobs),
+        texts = []
+        for j in jobs:
+            r = sched.results.get(j["id"], {}).get("result") or {}
+            texts.append(((r.get("message") or {}).get("content") or r.get("response") or "").encode("utf-8", "surrogatepass"))
+        return {"texts": texts, "wall": wall, "ok": ok, "chunks": chunks, "workers_used": used, "ticks": sched.ticks, "n": len(jobs),
                 "ttft_median_s": statistics.median(ttft) if ttft else None, "first_error": errs[0] if errs else None}
 
     loop = asyncio.new_event_loop()
@@ -618,7 +659,9 @@ def run_config3(args, N, path, rank, local_rank, world, dist, timed, peaks, extr
                                   "ttft_median_s": res[-1]["ttft_median_s"],
                                   "wall_tick0": {"tokens_per_s": gen_tokens / wall_s, "seconds_per_step": wall_s / args.steps},
                                   "wall_tick1s": {"tokens_per_s": tick1["n"] * N_GEN / tick1["wall"], "seconds": tick1["wall"], "ticks": tick1["ticks"],
-                                                  "note": "the reference's 1 000 ms dispatch tick (JobScheduler.ts:128-135), MAX_CONCURRENT_JOBS_PER_WORKER = batch"}}}}
+                                                  "note": "the reference's 1 000 ms dispatch tick (JobScheduler.ts:128-135), MAX_CONCURRENT_JOBS_PER_WORKER = batch"}}},
+            "dump": {"response_bytes": np.frombuffer(b"".join(res[-1]["texts"]), np.uint8),
+                     "response_lengths": np.array([len(t) for t in res[-1]["texts"]])}}
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -630,9 +673,12 @@ def run_config4(args, N, path, rank, local_rank, world, dist, timed, peaks, extr
     for w in range(max(1, args.warmup)):
         eng.generate(prompt_for(77_000 + w, T), num_predict=1, ignore_eos=True)
 
+    last = []
+
     def region():
         dev_ns = wall = launches = 0
         for i in range(args.steps):
+            last.clear()
             for s in range(S):
                 p = prompt_for(2000 + multirank.request_seeds(rank, i, 1)[0] * S + s, T)
                 t0 = time.perf_counter()
@@ -640,6 +686,7 @@ def run_config4(args, N, path, rank, local_rank, world, dist, timed, peaks, extr
                 wall += time.perf_counter() - t0
                 dev_ns += g.stats.prompt_eval_duration_ns
                 launches += g.stats.kernel_launches
+                last.append(g)
         return dev_ns, wall, launches
     (dev_ns, wall_s, launches), clocks = timed(region)
     tokens = float(args.steps * S * T)
@@ -650,14 +697,15 @@ def run_config4(args, N, path, rank, local_rank, world, dist, timed, peaks, extr
     achieved = flops_seq * S * args.steps / (dev_ns * 1e-9) / 1e12
     eng.close()
     return {"value": agg["value"], "ms_per_step": agg["device_s"] / args.steps * 1e3,
-            "dtype": "fp16 tensor cores (tcgen05, fp32 accumulate in TMEM); bf16 weights converted once at load (exact inside fp16's range)",
+            "dtype": "fp16 tensor cores (wgmma, fp32 accumulate); bf16 weights converted once at load (exact inside fp16's range)",
             "e2e": {"value": agg["e2e"], "unit": "tokens/s", "h2d_bytes_per_step": S * (T * 4 + 64), "d2h_bytes_per_step": S * 72,
                     "api": "gl_generate(prompt 2048, num_predict 1) x 32 (C ABI, host buffers)"},
             "gpu_launches": launches,
             "roofline": {"bound": "tensor", "kernel": "gemm_tc5_kernel (the prefill's linear layers: > 90 % of the step's flops); whole prefill timed",
                          "achieved": achieved, "peak": peaks["tf"], "unit": "TFLOP/s", "frac": achieved / peaks["tf"], "peak_source": peaks["src"],
                          "algorithmic_flops_per_step": flops_seq * S, "traffic": None},
-            "clocks": clocks, "extra": {}}
+            "clocks": clocks, "extra": {},
+            "dump": {"ids": np.concatenate([g.ids for g in last]), "logprobs": np.concatenate([g.logprobs for g in last])}}
 
 
 def run_config5(args, N, path, rank, local_rank, world, dist, timed, peaks, extra):
@@ -671,9 +719,12 @@ def run_config5(args, N, path, rank, local_rank, world, dist, timed, peaks, extr
         return [prompt_for(base + j, DOC_TOKENS, 32000 - 1) for j in range(n)]
     eng.embed(docs(999, 0, pack))
 
+    last = []
+
     def region():
         dev_ns = wall = launches = n = 0
         for i in range(args.steps):
+            last.clear()
             k = 0
             while k < args.docs:
                 d = docs(i, k, min(pack, args.docs - k))
@@ -684,6 +735,7 @@ def run_config5(args, N, path, rank, local_rank, world, dist, timed, peaks, extr
                 launches += st.kernel_launches
                 n += len(d)
                 k += len(d)
+                last.append(np.asarray(emb))
         assert np.isfinite(emb).all()
         return dev_ns, wall, launches, n
     (dev_ns, wall_s, launches, n), clocks = timed(region)
@@ -701,7 +753,8 @@ def run_config5(args, N, path, rank, local_rank, world, dist, timed, peaks, extr
             "roofline": {"bound": "tensor", "kernel": "gemm_tc5_kernel (packed prompt pass); whole gl_embed device time", "achieved": achieved,
                          "peak": peaks["tf"], "unit": "TFLOP/s", "frac": achieved / peaks["tf"], "peak_source": peaks["src"],
                          "algorithmic_flops_per_doc": flops_doc, "traffic": None},
-            "clocks": clocks, "extra": {"docs_per_call": pack}}
+            "clocks": clocks, "extra": {"docs_per_call": pack},
+            "dump": {"embeddings": np.concatenate(last)}}
 
 
 if __name__ == "__main__":

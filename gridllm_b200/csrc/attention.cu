@@ -32,7 +32,7 @@ __device__ __forceinline__ uint32_t attn_mapa(uint32_t local_smem_addr, uint32_t
 //             output that rank owns (st.shared::cluster into the rank's receive buffer: distributed shared memory) with its
 //             (max, sum); one cluster barrier; every rank merges its slice of the head group's output -- no global round trip,
 //             no ticket, and the merge is spread over the cluster (the ticket path: partial store 0.9 us + ticket 0.8 us + the
-//             last CTA's 32 partial loads 2.0 us per layer, profiles/r01_run59_perop_timeline.log).
+//             last CTA's 32 partial loads 2.0 us per layer).
 template <int DPL, bool CL>   // dims per lane = head_dim / 32
 __global__ void __launch_bounds__(32 * MAX_GRP) attn_decode_kernel(const __grid_constant__ AttnParams p) {
     constexpr int HD = DPL * 32;

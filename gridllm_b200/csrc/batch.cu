@@ -187,7 +187,7 @@ __global__ void __launch_bounds__(32 * B_MAX_GRP) batch_attn_kernel(const __grid
 
 // ---- the same attention on the tensor cores (mma.sync m16n8k16) --------------------------------------------------------------
 // The kernel above spends ~560 instructions per (page, query head): with B = 32 sequences at 576 tokens that is 20 M warp
-// instructions per layer, 39 us of a step in which the KV bytes themselves need 12 us (profiles/r02_runC).  Here ONE warp serves
+// instructions per layer, 39 us of a step in which the KV bytes themselves need 12 us.  Here ONE warp serves
 // all the query heads of a KV head at once: the GQA group is the M dimension of the MMA (rows = query heads, padded to 16),
 // S = Q K^T and O += P V are 32 tensor-core instructions per 16-token page instead of ~2 000 scalar ones.
 //   grid (KV head, split, row), 4 warps; the CTA's pages (split s: pages s, s + S, ...) are dealt round-robin to the warps;

@@ -1,5 +1,5 @@
-// Device helpers shared by the sm_100a kernels: mbarrier / TMA-bulk PTX, programmatic dependent
-// launch, warp reductions.  sm_100a only -- there is no fallback path.
+// Device helpers shared by the sm_90a kernels: mbarrier / TMA-bulk PTX, programmatic dependent
+// launch, warp reductions.  sm_90a only -- there is no fallback path.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>

@@ -1,5 +1,5 @@
 // Engine implementation: GGUF -> HBM upload (engine row layouts), paged KV pool, decode-step
-// construction (fused sm_100a kernels, PDL, CUDA graph) and the generate / embed drivers.
+// construction (fused sm_90a kernels, PDL, CUDA graph) and the generate / embed drivers.
 // See engine.h / include/gridllm_native.h for the reference call sites this replaces.
 #include "engine.h"
 
@@ -156,7 +156,7 @@ Status Engine::load(const std::string& path, int device, const gl_engine_opts* o
     CU(cudaSetDevice(device));
     cudaDeviceProp prop{};
     CU(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) return fail(GL_ERR_UNSUPPORTED, std::string("device '") + prop.name + "' is sm_" + std::to_string(prop.major * 10 + prop.minor) + "; this library is built for sm_100a (B200) only");
+    if (prop.major != 9) return fail(GL_ERR_UNSUPPORTED, std::string("device '") + prop.name + "' is sm_" + std::to_string(prop.major * 10 + prop.minor) + "; this library is built for sm_90a (H100) only");
     sm_count_ = prop.multiProcessorCount;
 
     abits_ = (opts && opts->act_bits == 8) ? 8 : 16;
@@ -184,7 +184,6 @@ Status Engine::load(const std::string& path, int device, const gl_engine_opts* o
     prefill_tc5_ = env_int("GL_PREFILL_TC5", 1) != 0;
     prefill_flash_ = env_int("GL_PREFILL_FLASH", 1) != 0;
     prefill_fuse_rope_ = env_int("GL_PREFILL_FUSE_ROPE", 1) != 0;
-    prefill_attn_tc5_ = env_int("GL_PREFILL_ATTN_TC5", 1) != 0;      // head dim 128; head dim 64 takes the mma.sync kernel
 
     std::string err = gguf_.open(path);
     if (!err.empty()) return fail(err.find("cannot open") == 0 ? GL_ERR_IO : GL_ERR_FORMAT, err);
@@ -235,7 +234,6 @@ Status Engine::load(const std::string& path, int device, const gl_engine_opts* o
     CU(prefill_configure());
     CU(gemm_tc5_configure());
     CU(flash_prefill_configure());
-    CU(flash_tc5_configure());
     CU(attn_decode_configure());
     if (attn_cluster_ && !attn_cluster_ok(n_head_, n_kv_, hd_, attn_splits_)) attn_cluster_ = false;      // shapes the slices do not fit: the ticket path
 
@@ -370,7 +368,7 @@ Status Engine::load(const std::string& path, int device, const gl_engine_opts* o
     ST(kv_reset());
     if (prefill_mode_ != 1) ST(build_prefill_weights());
     // the persistent single-launch decode kernel is opt-in: it is correct (same tests) but, as of round 1, slower than
-    // the per-op graph path (3.2 vs 2.3 ms/token; profiles/README.md)
+    // the per-op graph path
     if (fused_ && all_quant_ && env_int("GL_MEGA", 0) != 0) ST(build_mega());
     if (use_graph_ && !use_mega_) ST(build_graphs());
     CU(cudaStreamSynchronize(stream_));
@@ -1141,7 +1139,7 @@ Status Engine::gemv_tensor(const std::string& name, const float* x, float* y, in
     CU(cudaMalloc((void**)&dy, (size_t)m->rows * 4));
     CU(cudaMemcpy(dx, x, (size_t)m->cols * 4, cudaMemcpyHostToDevice));
     if (flush && !flush_buf_) {
-        flush_elems_ = (size_t)64 << 20;     // 256 MB > 126 MB L2
+        flush_elems_ = (size_t)64 << 20;     // 256 MB > 50 MB L2
         CU(cudaMalloc((void**)&flush_buf_, flush_elems_ * 4));
         allocs_.push_back(flush_buf_);
         CU(cudaMemset(flush_buf_, 0, flush_elems_ * 4));

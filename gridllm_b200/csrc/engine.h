@@ -1,4 +1,4 @@
-// Engine: one loaded GGUF model on one B200.  Owns the weights in HBM (engine row layouts), the
+// Engine: one loaded GGUF model on one H100.  Owns the weights in HBM (engine row layouts), the
 // paged KV pool, the device-resident step state and the captured decode-step CUDA graphs.
 // This is the native replacement for what sits behind OllamaService in the reference
 // (/root/reference/client/src/services/OllamaService.ts) -- see include/gridllm_native.h.
@@ -125,7 +125,7 @@ private:
     bool all_quant_ = true;
 
     // options
-    int device_ = 0, sm_count_ = 148;
+    int device_ = 0, sm_count_ = 132;
     int abits_ = 16;
     int nw_ = 12;              // consumer warps per CTA of the GEMV / persistent kernels
     int ring_depth_ = 2;       // ring slots per consumer warp (track depth, gemv_core.cuh)
@@ -143,7 +143,6 @@ private:
     int prefill_mode_ = 0, prefill_min_ = 8;
     bool have_w16_ = false, prefill_bf16_ = false, prefill_tc5_ = true;
     bool prefill_fuse_rope_ = true;  // RoPE / split / cache append in the QKV GEMM's epilogue (GL_PREFILL_FUSE_ROPE=0: the stand-alone kernel)
-    bool prefill_attn_tc5_ = true;   // the fused prompt attention on tcgen05 / tensor memory (prefill_attn_tc5.cu, head dim 128); GL_PREFILL_ATTN_TC5
     bool prefill_flash_ = true;     // fused prompt attention (prefill_attn.cu); GL_PREFILL_FLASH=0: the three-launch path, for A/B runs
     // prefill scratch (grown on demand)
     int pf_cap_ = 0;

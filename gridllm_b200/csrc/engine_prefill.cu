@@ -22,7 +22,7 @@ Status failp(int code, const std::string& m) { return Status{code, m}; }
 }  // namespace
 
 // Resident 16-bit copy of every layer matrix, dequantised on the GPU from the engine layouts.
-// 2 bytes/weight (16 GB for Llama-3-8B) of the 180 GB HBM buys a prefill that never touches the
+// 2 bytes/weight (16 GB for Llama-3-8B) of the 80 GB HBM buys a prefill that never touches the
 // 4-bit decode layout.  fp16 is used for every model type (what ggml's CUDA backend also does for
 // batched matmuls [external]); bf16 weights convert to fp16 exactly within fp16's normal range.
 Status Engine::build_prefill_weights() {
@@ -94,7 +94,7 @@ Status Engine::prefill_batched(int n, int* n_launch) {
     cudaStream_t s = stream_;
     const bool bf = prefill_bf16_;
     int nl = 0;
-    // linear layers: tcgen05 / TMEM / TMA GEMM (prefill_tc5.cu); GL_PREFILL_TC5=0 keeps the mma.sync kernel for A/B runs
+    // linear layers: wgmma / TMA GEMM (prefill_tc5.cu); GL_PREFILL_TC5=0 keeps the mma.sync kernel for A/B runs
     auto linear = [&](const GemmParams& g) -> cudaError_t {
         if (prefill_tc5_ && gemm_tc5_supported(g)) return gemm_tc5_launch(g, tp, bf, s);
         return gemm_tn_launch(g, bf, s);
@@ -126,8 +126,7 @@ Status Engine::prefill_batched(int n, int* n_launch) {
         if (prefill_flash_) {
             // (RoPE + split + cache append, then) ONE fused attention launch (prefill_attn.cu): scores stay on the SM
             if (!roped) { CU(rope_split_segs_launch(pf_qkv_, TP, n_head_, n_kv_, hd_, rope_cos_, rope_sin_, pf_q_, pf_k_, pf_vt_, kc, vc, tp, segs, s)); ++nl; }
-            if (prefill_attn_tc5_ && flash_tc5_supported(hd_)) CU(flash_tc5_launch(pf_q_, pf_k_, pf_vt_, (__half*)pf_attn_, segs, n_head_, n_kv_, hd_, tp, tp, scale, s));
-            else CU(flash_prefill_launch(pf_q_, pf_k_, pf_vt_, (__half*)pf_attn_, segs, n_head_, n_kv_, hd_, tp, scale, s));
+            CU(flash_prefill_launch(pf_q_, pf_k_, pf_vt_, (__half*)pf_attn_, segs, n_head_, n_kv_, hd_, tp, scale, s));
             ++nl;
         } else {
             CU(rope_split_launch(pf_qkv_, T, tp, 0, n_head_, n_kv_, hd_, rope_cos_, rope_sin_, pf_q_, pf_k_, pf_vt_, kc, vc, page_table_, tp, s)); ++nl;
@@ -238,8 +237,7 @@ Status Engine::prefill_packed(const std::vector<int>& starts, const std::vector<
                     CU(rope_split_segs_launch(pf_qkv_ + (size_t)row_lo * ldq, row_hi - row_lo, n_head_, n_kv_, hd_, rope_cos_, rope_sin_, pf_q_ + (size_t)row_lo * qd,
                                               pf_k_ + (size_t)row_lo * kvd, pf_vt_ + row_lo, kc, vc, tp, rs, s)); ++nl;
                 }
-                if (prefill_attn_tc5_ && flash_tc5_supported(hd_)) CU(flash_tc5_launch(pf_q_, pf_k_, pf_vt_, (__half*)pf_attn_, segs, n_head_, n_kv_, hd_, tp, tp, scale, s));
-                else CU(flash_prefill_launch(pf_q_, pf_k_, pf_vt_, (__half*)pf_attn_, segs, n_head_, n_kv_, hd_, tp, scale, s));
+                CU(flash_prefill_launch(pf_q_, pf_k_, pf_vt_, (__half*)pf_attn_, segs, n_head_, n_kv_, hd_, tp, scale, s));
                 ++nl;
             }
         } else

@@ -1,4 +1,4 @@
-// Decode GEMV: y = dequant(W)[rows x K] * x[K], the kernel that bounds Llama decode on B200.
+// Decode GEMV: y = dequant(W)[rows x K] * x[K], the kernel that bounds Llama decode on H100.
 //
 // Replaces the quantised mat-vec that, in the reference, runs inside the Ollama daemon behind
 // OllamaService.generateResponse / generateStreamResponse
@@ -255,7 +255,7 @@ __global__ void __launch_bounds__(256) gemv_fp_kernel(const uint8_t* __restrict_
 
 cudaError_t gemv_fp_launch(const void* w, int type, int rows, int cols, const float* x, float* y, cudaStream_t s) {
     if (cols % 8) return cudaErrorInvalidValue;
-    const int blocks = min((rows + 7) / 8, 148 * 8);
+    const int blocks = min((rows + 7) / 8, 132 * 8);
     const uint8_t* wb = static_cast<const uint8_t*>(w);
     switch (type) {
         case T_F32: gemv_fp_kernel<T_F32><<<blocks, 256, 0, s>>>(wb, rows, cols, x, y); break;

@@ -23,7 +23,7 @@
 //
 // Why small slots: the bytes a SM keeps in flight are what the HBM pipe needs (~48-64 KB per SM at 6.5 TB/s x ~1 us),
 // and nothing more -- every extra prefetched byte sits in the SM's request FIFO in front of the latency-critical
-// loads of a phase change (barrier flag, x), which is what profiles/r01_run19_mega_trace_inflight.log measured
+// loads of a phase change (barrier flag, x), which is what a timeline of the persistent kernel measured
 // (prologue 3.2 us at 72 KB in flight, 4.5 us at 144-180 KB).
 #pragma once
 #include "common.cuh"
@@ -335,17 +335,14 @@ __device__ __forceinline__ void gemv_prologue_static_hb(const GemvParams& p, int
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Prologue, half block per thread straight from global memory with 256-BIT LOADS (ld.global.v8.f32, SASS LDG.E.256,
-// new on sm_100): a lane's 16 columns are two whole 32-byte sectors, so the load requests are as few as in the coalesced
-// float4 version (the LDG.128 attempt doubled them and x arrived after 3.2 us, run 46) while the arithmetic keeps the
-// half-block form: one shuffle for the block maximum, one for the block sum, reciprocal / addresses / stores once per 16
-// columns.  Serves every width: K = 14336 is 896 half blocks = 2.3 per thread, all of them requested at once.
+// Prologue, half block per thread straight from global memory: a lane's 16 columns are two whole 32-byte sectors, each read
+// with two back-to-back 128-bit loads (Hopper has no 256-bit global load), while the arithmetic keeps the half-block form: one
+// shuffle for the block maximum, one for the block sum, reciprocal / addresses / stores once per 16 columns.  Serves every
+// width: K = 14336 is 896 half blocks = 2.3 per thread, all of them requested at once.
 // ---------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void ldcg256(const float* p, float* v) {
-    asm volatile("ld.global.cg.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-                 : "l"(p)
-                 : "memory");
+    asm volatile("ld.global.cg.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]) : "l"(p) : "memory");
+    asm volatile("ld.global.cg.v4.f32 {%0, %1, %2, %3}, [%4 + 16];" : "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]) : "l"(p) : "memory");
 }
 
 template <int ABITS, int NW>

@@ -1,4 +1,4 @@
-// Launcher interface of the sm_100a kernels (implemented in gemv.cu, attention.cu, misc.cu,
+// Launcher interface of the sm_90a kernels (implemented in gemv.cu, attention.cu, misc.cu,
 // prefill.cu).  Host code (engine.cu) only sees plain structs and cudaStream_t.
 #pragma once
 #include <cuda_fp16.h>

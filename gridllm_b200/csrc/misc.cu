@@ -317,7 +317,7 @@ cudaError_t pool_embedding_launch(const float* h, int rows, int n, const float* 
 }
 
 cudaError_t l2_flush_launch(float* buf, size_t n, cudaStream_t s) {
-    l2_flush_kernel<<<148 * 4, 256, 0, s>>>(buf, n);
+    l2_flush_kernel<<<132 * 4, 256, 0, s>>>(buf, n);
     return cudaGetLastError();
 }
 

@@ -5,11 +5,11 @@
 // OllamaService.generate*Response / generateEmbedding
 // (/root/reference/client/src/services/OllamaService.ts:142-145, 235-237, 633-636).
 //
-// Round-1 implementation: a TN GEMM  C[M x N] = A[M x K] * B[N x K]^T  on 16-bit inputs with fp32
-// accumulation (mma.sync m16n8k16 -- the legacy HMMA tensor path; the tcgen05/TMEM version is the next
-// step, DESIGN.md section 8), cp.async 3-stage pipeline, XOR-swizzled shared memory, ldmatrix fragments,
-// fused epilogues (residual add, SiLU*mul).  Weights are dequantised once at load into a resident
-// 16-bit copy (HBM is 180 GB; 16 GB for Llama-3-8B).  Attention over the prompt is two batched GEMMs
+// The general GEMM: a TN GEMM  C[M x N] = A[M x K] * B[N x K]^T  on 16-bit inputs with fp32 accumulation
+// (mma.sync m16n8k16; the plain linear layers run on the TMA + wgmma kernel of prefill_tc5.cu), cp.async
+// 3-stage pipeline, XOR-swizzled shared memory, ldmatrix fragments, fused epilogues (residual add,
+// SiLU*mul).  Weights are dequantised once at load into a resident 16-bit copy (HBM is 80 GB; 16 GB for
+// Llama-3-8B).  Attention over the prompt is two batched GEMMs
 // (Q K^T, P V) around a causal softmax.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -384,7 +384,7 @@ cudaError_t gemm_tn_launch(const GemmParams& p, bool bf16, cudaStream_t s) {
 
 cudaError_t dequant_rows_launch(const uint8_t* src, int type, int rows, int cols, int row_stride, int tile_rows, void* dst, int dst_ld, int dst_row0,
                                 int interleave, bool bf16, cudaStream_t s) {
-    const int blocks = rows < 148 * 8 ? rows : 148 * 8;
+    const int blocks = rows < 132 * 8 ? rows : 132 * 8;
     if (bf16) dequant_rows_kernel<__nv_bfloat16><<<blocks, 256, 0, s>>>(src, type, rows, cols, row_stride, tile_rows, (__nv_bfloat16*)dst, dst_ld, dst_row0, interleave);
     else dequant_rows_kernel<__half><<<blocks, 256, 0, s>>>(src, type, rows, cols, row_stride, tile_rows, (__half*)dst, dst_ld, dst_row0, interleave);
     return cudaGetLastError();

@@ -11,7 +11,7 @@ enum GemmEpilogue : int {
     GEMM_EPI_ADD_F32 = 1,  // C fp32 += acc                 (residual add in place)
     GEMM_EPI_T16 = 2,      // C 16-bit = acc
     GEMM_EPI_SILU = 3,     // B rows interleaved [8 gate | 8 up]: C16[m][col] = silu(gate) * up
-    GEMM_EPI_ROPE_SPLIT = 4,  // the QKV projection: RoPE on the q / k columns, 16-bit Q / K rows, V^T columns, fp16 cache pages (tcgen05 path only)
+    GEMM_EPI_ROPE_SPLIT = 4,  // the QKV projection: RoPE on the q / k columns, 16-bit Q / K rows, V^T columns, fp16 cache pages (prefill_tc5.cu only)
 };
 
 // The sequences of one prompt pass: sequence i owns rows [start[i], start[i] + len[i]) of the packed activation matrix (starts at
@@ -56,7 +56,7 @@ struct GemmParams {
 
 cudaError_t prefill_configure();   // per device: opt in to the GEMM's dynamic shared memory
 cudaError_t gemm_tn_launch(const GemmParams& p, bool bf16, cudaStream_t s);      // mma.sync path (batched attention GEMMs)
-// tcgen05 / TMEM / TMA path (prefill_tc5.cu) for the plain linear layers; a_rows_alloc = rows of A that exist in memory
+// wgmma / TMA path (prefill_tc5.cu) for the plain linear layers; a_rows_alloc = rows of A that exist in memory
 cudaError_t gemm_tc5_configure();
 bool gemm_tc5_supported(const GemmParams& p);
 cudaError_t gemm_tc5_launch(const GemmParams& p, int a_rows_alloc, bool bf16, cudaStream_t s);
@@ -72,12 +72,6 @@ bool flash_prefill_supported(int hd);
 // out[rows][n_head * hd] = causal softmax(q k^T * scale) v per sequence and head; q / k rows, vt = V^T [n_kv * hd][vt_ld]
 cudaError_t flash_prefill_launch(const __half* q, const __half* k, const __half* vt, __half* out, const PrefillSegs& segs, int n_head, int n_kv,
                                  int hd, int vt_ld, float scale, cudaStream_t s);
-// the same on tcgen05 (prefill_attn_tc5.cu; head dim 128): scores, probabilities and the output accumulator in tensor memory.
-// rows_alloc = rows of q / k (columns of vt) that exist in memory (TMA reads beyond them as zeros)
-cudaError_t flash_tc5_configure();
-bool flash_tc5_supported(int hd);
-cudaError_t flash_tc5_launch(const __half* q, const __half* k, const __half* vt, __half* out, const PrefillSegs& segs, int n_head, int n_kv, int hd,
-                             int vt_ld, int rows_alloc, float scale, cudaStream_t s);
 // rope_split for every sequence of a pack in one launch (rows_pad = rows of the pack, padding rows are zeroed)
 cudaError_t rope_split_segs_launch(const float* qkv, int rows_pad, int n_head, int n_kv, int hd, const float* cos_t, const float* sin_t, __half* qo,
                                    __half* ko, __half* vt, __half* k_cache, __half* v_cache, int vt_ld, const PrefillSegs& segs, cudaStream_t s);

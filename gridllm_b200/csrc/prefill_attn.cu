@@ -2,12 +2,12 @@
 // 128-row query tile, scores never leave the SM.  Replaces the three launches per sequence and layer of the first
 // version (Q K^T GEMM -> fp32 scores in HBM -> causal softmax -> P in HBM -> P V GEMM: 1.2 GB of HBM traffic per layer
 // at 2 048 tokens) on the path behind OllamaService.generate*Response / generateEmbedding
-// (/root/reference/client/src/services/OllamaService.ts:142-145, 235-237, 633-636: the prompt-evaluation phase).
+// (client/src/services/OllamaService.ts of the reference project:142-145, 235-237, 633-636: the prompt-evaluation phase).
 //
 // Shape of the work: per (query head, 128-row query tile, sequence) one CTA of four warps, 32 query rows per warp,
 // KV tiles of 64 rows.  This version keeps the accumulators in registers (mma.sync m16n8k16, fp32 accumulate) and
-// spends its effort on what the old path wasted: HBM traffic and launches.  It serves head dim 64 and is the A/B
-// partner of the tcgen05 kernel (prefill_attn_tc5.cu, head dim 128: scores, probabilities and output in tensor memory).  K rows [kv][hd] and V^T rows [hd][kv] (what rope_split writes) are
+// spends its effort on what the old path wasted: HBM traffic and launches.  It serves head dims 64 and 128.  K rows [kv][hd] and
+// V^T rows [hd][kv] (what rope_split writes) are
 // both "n-major with k contiguous", i.e. the B operand of a TN product: plain ldmatrix for both products, no
 // transposes.  cp.async double buffering of the K / V^T tiles, XOR-swizzled shared memory, 96 KB per CTA at head dim
 // 128: two CTAs per SM.  A pack of sequences (block-diagonal causal attention, section 4.7 of DESIGN.md) is one launch:

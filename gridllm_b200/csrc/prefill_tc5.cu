@@ -1,22 +1,19 @@
-// Batched-prefill linear layers on the 5th-generation tensor cores: C[M x N] = A[M x K] * B[N x K]^T, 16-bit inputs,
-// fp32 accumulation in TENSOR MEMORY.  This is the one place on the hot path where the work is a true dense
-// contraction (north_star): the prompt's [T x n_embd] activations against each resident 16-bit weight matrix.
-// Reference call site: the prompt-evaluation phase inside Ollama behind OllamaService.generate*Response /
-// generateEmbedding (/root/reference/client/src/services/OllamaService.ts:142-145, 235-237, 633-636).
+// Batched-prefill linear layers on the Hopper tensor cores: C[M x N] = A[M x K] * B[N x K]^T, 16-bit inputs, fp32 accumulation
+// in registers (wgmma).  This is the one place on the hot path where the work is a true dense contraction: the prompt's
+// [T x n_embd] activations against each resident 16-bit weight matrix.
+// Reference call site: the prompt-evaluation phase inside Ollama behind OllamaService.generate*Response / generateEmbedding
+// (client/src/services/OllamaService.ts:142-145, 235-237, 633-636 of the reference project).
 //
-// Shape of the kernel (persistent: one CTA per SM walks 128 x 128 output tiles, 6 warps, everything asynchronous,
-// hand-written PTX; the accumulator is double-buffered in TMEM, so the epilogue of tile i overlaps the MMAs of tile i+1
-// and the TMA ring never drains between tiles):
-//   warp 0 / one lane : TMA producer -- cp.async.bulk.tensor.2d of a 128 x 64 A box and a 128 x 64 B box per K-step
-//                       into a 6-stage mbarrier ring (128-byte swizzle, 32 KB per stage);
-//   warp 1 / one lane : MMA issuer   -- per stage four tcgen05.mma.cta_group::1.kind::f16 (M128 N128 K16), operands
-//                       addressed by shared-memory matrix descriptors, accumulator = 128 of the CTA's 256 TMEM columns
-//                       (tiles alternate between the two halves); tcgen05.commit hands the stage back to the producer and,
-//                       after the last K-step of a tile, wakes the epilogue;
-//   warps 2..5        : epilogue     -- tcgen05.ld 32 lanes x 32 columns at a time (warp w may touch TMEM lanes
-//                       32*(w%4)..), fused epilogue (fp32 store, residual add, 16-bit store, SiLU*mul), global stores;
-//                       then hands the accumulator half back to the MMA issuer (acc_empty).
-// SASS to look for: UTCHMMA (tcgen05.mma), UTMALDG (TMA), LDTM (tcgen05.ld), UTCBAR (tcgen05.commit).
+// Shape of the kernel (persistent: one CTA per SM walks 128 x 128 output tiles, three warpgroups, hand-written PTX):
+//   warpgroup 0, one lane : TMA producer -- cp.async.bulk.tensor.2d of a 128 x 64 A box and a 128 x 64 B box per K-step into a
+//                           4-stage mbarrier ring (128-byte swizzle, 32 KB per stage); the ring runs on across tile boundaries;
+//   warpgroups 1, 2       : consumers -- warpgroup c owns rows 64c..64c+63 of the tile: per stage four wgmma.m64n128k16
+//                           (operands addressed by shared-memory matrix descriptors, accumulator in 64 registers per thread),
+//                           the stage goes back to the producer once the MMAs that read it have completed; after the last
+//                           K-step the accumulator is staged through shared memory so that each thread owns 32 consecutive
+//                           columns of one row, and the fused epilogue (fp32 store, residual add, 16-bit store, SiLU*mul,
+//                           RoPE / split) writes global memory.
+// SASS to look for: HGMMA (wgmma), UTMALDG (TMA).
 #include <cuda.h>
 #include <algorithm>
 #include <cstdlib>
@@ -26,31 +23,21 @@
 #include "common.cuh"
 #include "kernels.h"
 #include "prefill.h"
+#include "wgmma.cuh"
 
 namespace gl {
 
 namespace {
 
-constexpr int BM = 128, BK = 64;
-constexpr int UMMA_K = 16;
-constexpr int TILE_A_BYTES = BM * BK * 2;
-constexpr int TC5_THREADS = 192;
-constexpr int ACC_BUFS = 2;
-// Output tile 128 x BN.  BN = 128: 6 stages of 32 KB, accumulators in 256 of the SM's 512 TMEM columns.  BN = 256: 4 stages of
-// 48 KB, accumulators in all 512 columns -- each K-step then stages 48 KB for 128 x 256 x 64 MACs (96 B per MMA cycle instead
-// of 128): the L2 -> shared-memory feed, not the tensor pipe, is what limits the 128 x 128 tile (tensor pipe active 46 %, run 59).
-// PAIR = 2: two CTAs on the two SMs of a TPC (a cluster of two) share one 256 x BN tile -- tcgen05.mma.cta_group::2, M 256: each CTA
-// stages its own 128 rows of A and HALF of the B tile (BN / 2 weight rows), the tensor cores of both SMs read both halves of B.
-// Per SM and K-step that is 32 KB staged for 128 x 256 x 64 MACs instead of 48 KB: the shared-memory port (TMA writes + operand
-// reads), which is what limits the one-CTA 128 x 256 tile, carries 128 B per MMA cycle instead of 192, and 6 stages fit.
-template <int BN, int PAIR> struct Tc5Cfg {
-    static constexpr int B_ROWS = BN / PAIR;                     // rows of B this CTA stages
-    static constexpr int STAGES = (BN == 128 || PAIR == 2) ? 6 : 4;
-    static constexpr int TILE_B_BYTES = B_ROWS * BK * 2;
-    static constexpr int STAGE_BYTES = TILE_A_BYTES + TILE_B_BYTES;
-    static constexpr int TMEM_COLS = ACC_BUFS * BN;
-    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 /* alignment slack */ + 256 /* barriers */;
-};
+constexpr int BM = 128, BN = 128, BK = 64;
+constexpr int WG_K = 16;
+constexpr int TILE_A_BYTES = BM * BK * 2, TILE_B_BYTES = BN * BK * 2;
+constexpr int STAGE_BYTES = TILE_A_BYTES + TILE_B_BYTES;
+constexpr int STAGES = 4;
+constexpr int TC_THREADS = 384;
+constexpr int STG_LD = BN + 4;                 // staging row stride in floats: float4 reads of 8 consecutive rows hit 8 distinct bank quads
+constexpr size_t STG_BYTES = (size_t)BM * STG_LD * 4;
+constexpr size_t TC_SMEM = (size_t)STAGES * STAGE_BYTES + STG_BYTES + 1024 /* alignment slack */ + 256 /* barriers */;
 
 struct Tc5Params {
     CUtensorMap ta;      // A: dims {K, M_alloc}, box {64, 128}, 128-B swizzle
@@ -66,84 +53,6 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(dst)),
                  "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
                  : "memory");
-}
-__device__ __forceinline__ void tc5_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc5_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ bool tc5_elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P1;\n\telect.sync _|P1, 0xffffffff;\n\tselp.b32 %0, 1, 0, P1;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tc5_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void tc5_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// ---- CTA pair (cta_group::2) -----------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t tc5_cluster_rank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void tc5_cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// the same shared-memory location in CTA 0 of the pair: bit 24 of a shared::cluster address is the rank inside the pair
-constexpr uint32_t TC5_PEER_MASK = 0xFEFFFFFFu;
-// TMA of a CTA of a pair: the bytes land in THIS CTA's shared memory, the transaction count on the LEADER's mbarrier
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-                     smem_u32(dst)),
-                 "l"(map), "r"(smem_u32(bar) & TC5_PEER_MASK), "r"(c0), "r"(c1)
-                 : "memory");
-}
-// commit of the pair's MMAs: one arrival on the mbarrier at this offset in BOTH CTAs
-__device__ __forceinline__ void tc5_commit_pair(uint64_t* bar) {
-    const uint16_t mask = 3;
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)), "h"(mask)
-                 : "memory");
-}
-__device__ __forceinline__ void tc5_mma_f16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrival on the mbarrier at this offset in the LEADER's shared memory (from either CTA of the pair)
-__device__ __forceinline__ void tc5_arrive_leader(uint64_t* bar) {
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(bar)), "r"(0u));
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
-}
-
-// K-major operand tile, 128-byte swizzle, rows of 64 16-bit elements (one swizzle atom = 8 rows x 128 B = 1024 B):
-// start address, stride between 8-row groups = 1024 B, descriptor version 1 (sm_100), layout SWIZZLE_128B
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-// 32 lanes x 32 columns of fp32: thread t of the warp receives row (lane base + t), 32 consecutive columns
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t* v) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]),
-          "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-          "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]),
-          "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
 template <typename T> __device__ __forceinline__ T cvt16(float v);
@@ -261,178 +170,124 @@ __device__ __forceinline__ void epilogue_rope_split(const RopeSplitArgs& a, int 
     }
 }
 
-template <int BN, int PAIR>
-__global__ void __launch_bounds__(TC5_THREADS, 1) gemm_tc5_kernel(const __grid_constant__ Tc5Params p) {
-    using Cfg = Tc5Cfg<BN, PAIR>;
-    constexpr int STAGES = Cfg::STAGES, STAGE_BYTES = Cfg::STAGE_BYTES, B_ROWS = Cfg::B_ROWS;
-    constexpr int TMEM_COLS = Cfg::TMEM_COLS;
-    constexpr int TM = BM * PAIR;                     // rows of the tile a CTA (pair) owns
+template <bool BF16>
+__global__ void __launch_bounds__(TC_THREADS, 1) gemm_tc5_kernel(const __grid_constant__ Tc5Params p) {
     extern __shared__ uint8_t smem_raw[];
     // 128-byte-swizzled tiles must sit on 1024-byte boundaries
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)STAGES * STAGE_BYTES);
+    float* stg = reinterpret_cast<float*>(smem + (size_t)STAGES * STAGE_BYTES);     // [BM][STG_LD] accumulator staging
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)STAGES * STAGE_BYTES + STG_BYTES);
     uint64_t* empty = full + STAGES;
-    uint64_t* acc_full = empty + STAGES;          // [ACC_BUFS] MMA issuer -> epilogue
-    uint64_t* acc_empty = acc_full + ACC_BUFS;    // [ACC_BUFS] epilogue (4 warps per CTA) -> MMA issuer
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + ACC_BUFS);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int rank = PAIR == 2 ? (int)tc5_cluster_rank() : 0;      // CTA inside the pair; rank 0 issues the MMAs
-    const int worker = (int)blockIdx.x / PAIR, n_workers = (int)gridDim.x / PAIR;
+    const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+    const int warp = t >> 5, lane = t & 31;
     // M tiles are the fast grid dimension: the (few) CTAs that share a weight tile run back to back and find it in L2
-    // (N-major order re-read every weight byte from DRAM once per M tile: 943 MB for the 235 MB gate/up matrix, run 39)
-    const int tiles_m = (p.m + TM - 1) / TM, tiles_n = (p.n + BN - 1) / BN, n_tiles = tiles_m * tiles_n;
+    const int tiles_m = (p.m + BM - 1) / BM, tiles_n = (p.n + BN - 1) / BN, n_tiles = tiles_m * tiles_n;
     const int nk = (p.k + BK - 1) / BK;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&p.ta) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&p.tb) : "memory");
-    }
-    if (warp == 1 && lane == 0) {
         for (int i = 0; i < STAGES; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 1);
-        }
-        for (int i = 0; i < ACC_BUFS; ++i) {
-            mbar_init(&acc_full[i], 1);
-            mbar_init(&acc_empty[i], 4 * PAIR);
+            mbar_init(&empty[i], 2);        // one arrival per consumer warpgroup
         }
         fence_mbar_init();
     }
-    if (warp == 2) {   // one warp (of each CTA of a pair) allocates the accumulator's TMEM columns and publishes the base address
-        if constexpr (PAIR == 2) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-    }
-    tc5_fence_before();
     __syncthreads();
-    if constexpr (PAIR == 2) tc5_cluster_sync();      // the peer's barriers exist before anything signals them
-    tc5_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        if (lane == 0) {
-            // ===== TMA producer: the ring runs on across tile boundaries =====
+    if (wg == 0) {
+        if (t == 0) {
+            // ===== TMA producer =====
             int st = 0;
             uint32_t ph = 0;
-            for (int tile = worker; tile < n_tiles; tile += n_workers) {
-                const int m0 = (tile % tiles_m) * TM + rank * BM, n0 = (tile / tiles_m) * BN + rank * B_ROWS;
+            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+                const int m0 = (tile % tiles_m) * BM, n0 = (tile / tiles_m) * BN;
                 for (int kb = 0; kb < nk; ++kb) {
                     mbar_wait(&empty[st], ph ^ 1u);
                     uint8_t* sa = smem + (size_t)st * STAGE_BYTES;
-                    if constexpr (PAIR == 2) {
-                        // both CTAs' boxes are counted on the leader's barrier (armed by the leader alone: the phase cannot
-                        // complete before its arrival, however early the peer's bytes land)
-                        if (rank == 0) mbar_expect_tx(&full[st], 2 * STAGE_BYTES);
-                        tma_load_2d_pair(sa, &p.ta, kb * BK, m0, &full[st]);
-                        tma_load_2d_pair(sa + TILE_A_BYTES, &p.tb, kb * BK, n0, &full[st]);
-                    } else {
-                        mbar_expect_tx(&full[st], STAGE_BYTES);
-                        tma_load_2d(sa, &p.ta, kb * BK, m0, &full[st]);
-#pragma unroll
-                        for (int h = 0; h < BN / 128; ++h)      // the tensor map's box is 128 rows: a 256-row B tile is two boxes, 16 KB apart
-                            tma_load_2d(sa + TILE_A_BYTES + h * (128 * BK * 2), &p.tb, kb * BK, n0 + h * 128, &full[st]);
-                    }
+                    mbar_expect_tx(&full[st], STAGE_BYTES);
+                    tma_load_2d(sa, &p.ta, kb * BK, m0, &full[st]);
+                    tma_load_2d(sa + TILE_A_BYTES, &p.tb, kb * BK, n0, &full[st]);
                     if (++st == STAGES) { st = 0; ph ^= 1u; }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer (of a pair: the leader's) =====
-        // The whole warp walks the loop with warp-uniform values and ONE ELECTED lane issues: inside `if (lane == 0)` the
-        // compiler cannot keep descriptors and addresses in uniform registers and wraps every tcgen05 instruction in a
-        // convert-to-uniform loop (ELECT / R2UR / UTCHMMA / BRA.U.ANY); written this way an MMA is two uniform adds and the
-        // instruction (found on the batched decode GEMM, where the issuer's own instruction stream set the pace: qgemm.cu).
-        // instruction descriptor: D = F32, A / B = F16 or BF16, both K-major, N = BN, M = 128 (pair: 256)
-        if (rank == 0) {
-            const uint32_t fmt = p.bf16 ? 1u : 0u;
-            const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-            const uint32_t tb = __shfl_sync(0xffffffffu, tmem_base, 0);
-            const uint32_t smem0 = __shfl_sync(0xffffffffu, smem_u32(smem), 0);
-            int st = 0;
-            uint32_t ph = 0;
-            int it = 0;
-            for (int tile = worker; tile < n_tiles; tile += n_workers, ++it) {
-                const int buf = it & 1;
-                const uint32_t aph = (uint32_t)(it >> 1) & 1u;
-                mbar_wait(&acc_empty[buf], aph ^ 1u);      // the epilogue(s) have drained this half (free on its first use)
-                tc5_fence_after();
-                const uint32_t tmem_d = tb + (uint32_t)(buf * BN);
-                for (int kb = 0; kb < nk; ++kb) {
-                    mbar_wait(&full[st], ph);
-                    tc5_fence_after();
-                    const uint32_t sa = smem0 + (uint32_t)(st * STAGE_BYTES);
-                    const uint64_t adesc = umma_desc_sw128(sa), bdesc = umma_desc_sw128(sa + TILE_A_BYTES);
-                    if (tc5_elect_one()) {
-#pragma unroll
-                        for (int k = 0; k < BK / UMMA_K; ++k) {
-                            // advancing K inside the swizzle atom: +32 bytes = +2 in the descriptor's 16-byte address units
-                            if constexpr (PAIR == 2) tc5_mma_f16_pair(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, k ? 1u : (kb ? 1u : 0u));
-                            else tc5_mma_f16(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, k ? 1u : (kb ? 1u : 0u));
-                        }
-                        if constexpr (PAIR == 2) {
-                            tc5_commit_pair(&empty[st]);                       // both CTAs' stages are free once these MMAs have read them
-                            if (kb == nk - 1) tc5_commit_pair(&acc_full[buf]); // ... and both halves of the accumulator are complete
-                        } else {
-                            tc5_commit(&empty[st]);                       // the stage is free once these MMAs have read it
-                            if (kb == nk - 1) tc5_commit(&acc_full[buf]); // ... and the accumulator is complete
-                        }
-                    }
-                    __syncwarp();
-                    if (++st == STAGES) { st = 0; ph ^= 1u; }
-                }
-            }
-        }
-    } else {
-        // ===== epilogue: TMEM -> registers -> global (each CTA of a pair: its own 128 rows) =====
-        const int q = warp & 3;                      // the TMEM lane quarter this warp may access
-        int it = 0;
-        for (int tile = worker; tile < n_tiles; tile += n_workers, ++it) {
-            const int m0 = (tile % tiles_m) * TM + rank * BM, n0 = (tile / tiles_m) * BN;
-            const int buf = it & 1;
-            mbar_wait(&acc_full[buf], (uint32_t)(it >> 1) & 1u);
-            tc5_fence_after();
-            const int row = m0 + q * 32 + lane;
-            int pos = -1;                               // GEMM_EPI_ROPE_SPLIT: the row's position inside its sequence (-1: padding)
-            const int* page_table = nullptr;
-            if (p.epi == GEMM_EPI_ROPE_SPLIT) {
-                for (int i = 0; i < p.rope.segs.n; ++i) {
-                    const int st = p.rope.segs.start[i], ln = p.rope.segs.len[i];
-                    if (row >= st && row < st + (ln + 127) / 128 * 128) {
-                        pos = row - st < ln ? row - st : -1;
-                        page_table = p.rope.segs.table[i];
-                    }
-                }
-            }
-#pragma unroll 1
-            for (int c = 0; c < BN / 32; ++c) {
-                uint32_t v[32];
-                tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BN + c * 32), v);
-                const int col0 = n0 + c * 32;
-                if (row < p.m && col0 < p.n) {
-                    if (p.epi == GEMM_EPI_ROPE_SPLIT) epilogue_rope_split(p.rope, row, pos, page_table, col0, v);
-                    else if (p.bf16) epilogue_row<__nv_bfloat16>(p, row, col0, v);
-                    else epilogue_row<__half>(p, row, col0, v);
-                }
-            }
-            tc5_fence_before();
-            __syncwarp();
-            if (lane == 0) {                          // this warp's quarter of the accumulator half is in registers / memory
-                if constexpr (PAIR == 2) tc5_arrive_leader(&acc_empty[buf]);
-                else mbar_arrive(&acc_empty[buf]);
-            }
-        }
+        return;
     }
-    tc5_fence_before();
-    __syncthreads();
-    if constexpr (PAIR == 2) tc5_cluster_sync();      // neither CTA frees tensor memory the pair's MMAs may still write
-    if (warp == 2) {
-        if constexpr (PAIR == 2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
+
+    // ===== consumers: warpgroup c = wg - 1 computes rows 64c..64c+63 of each tile =====
+    const int c = wg - 1;
+    const uint32_t smem0 = smem_u32(smem);
+    float* my_stg = stg + (size_t)(64 * c) * STG_LD;
+    int st = 0;
+    uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const int m0 = (tile % tiles_m) * BM, n0 = (tile / tiles_m) * BN;
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        int prev = -1;
+        for (int kb = 0; kb < nk; ++kb) {
+            mbar_wait(&full[st], ph);
+            const uint32_t sa = smem0 + (uint32_t)(st * STAGE_BYTES);
+            const uint64_t adesc = wgmma_desc_sw128(sa + (uint32_t)(c * 64 * BK * 2)), bdesc = wgmma_desc_sw128(sa + TILE_A_BYTES);
+            wgmma_fence_acc<BN / 2>(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BK / WG_K; ++k) wgmma_m64k16<BN, BF16>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), 1u);
+            wgmma_commit();
+            // the MMAs of the previous stage have completed once at most this stage's group is outstanding: release that stage
+            wgmma_wait<1>();
+            wgmma_fence_acc<BN / 2>(acc);
+            if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
+            prev = st;
+            if (++st == STAGES) { st = 0; ph ^= 1u; }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_acc<BN / 2>(acc);
+        if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
+
+        // accumulator fragment -> staging rows (the previous tile's readers of this warpgroup are done: barrier first)
+        named_bar_sync(1 + c, 128);
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i) {
+            const int r = 16 * warp + (lane >> 2), col = 8 * i + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(my_stg + (size_t)r * STG_LD + col) = make_float2(acc[4 * i], acc[4 * i + 1]);
+            *reinterpret_cast<float2*>(my_stg + (size_t)(r + 8) * STG_LD + col) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+        }
+        named_bar_sync(1 + c, 128);
+
+        // epilogue: thread = one row (the 32 lanes of a warp are 32 consecutive rows), 32 consecutive columns per chunk
+        const int lr = (warp & 1) * 32 + lane, row = m0 + 64 * c + lr;
+        int pos = -1;                               // GEMM_EPI_ROPE_SPLIT: the row's position inside its sequence (-1: padding)
+        const int* page_table = nullptr;
+        if (p.epi == GEMM_EPI_ROPE_SPLIT) {
+            for (int i = 0; i < p.rope.segs.n; ++i) {
+                const int s0 = p.rope.segs.start[i], ln = p.rope.segs.len[i];
+                if (row >= s0 && row < s0 + (ln + 127) / 128 * 128) {
+                    pos = row - s0 < ln ? row - s0 : -1;
+                    page_table = p.rope.segs.table[i];
+                }
+            }
+        }
+#pragma unroll 1
+        for (int j = 0; j < 2; ++j) {
+            const int ch = (warp >> 1) * 2 + j;
+            uint32_t v[32];
+            const float4* src = reinterpret_cast<const float4*>(my_stg + (size_t)lr * STG_LD + ch * 32);
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+                const float4 f = src[q];
+                v[4 * q] = __float_as_uint(f.x); v[4 * q + 1] = __float_as_uint(f.y); v[4 * q + 2] = __float_as_uint(f.z); v[4 * q + 3] = __float_as_uint(f.w);
+            }
+            const int col0 = n0 + ch * 32;
+            if (row < p.m && col0 < p.n) {
+                if (p.epi == GEMM_EPI_ROPE_SPLIT) epilogue_rope_split(p.rope, row, pos, page_table, col0, v);
+                else if (BF16) epilogue_row<__nv_bfloat16>(p, row, col0, v);
+                else epilogue_row<__half>(p, row, col0, v);
+            }
+        }
     }
 }
 
@@ -462,12 +317,12 @@ bool make_map(CUtensorMap* map, const void* base, int rows, int k, int ld, bool 
               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+
 }  // namespace
 
 cudaError_t gemm_tc5_configure() {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc5_kernel<128, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Tc5Cfg<128, 1>::SMEM);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tc5_kernel<256, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Tc5Cfg<256, 1>::SMEM);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tc5_kernel<256, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Tc5Cfg<256, 2>::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(gemm_tc5_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tc5_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM);
     return e;
 }
 
@@ -489,52 +344,11 @@ cudaError_t gemm_tc5_launch(const GemmParams& p, int a_rows_alloc, bool bf16, cu
     tp.c = p.c; tp.m = p.m; tp.n = p.n; tp.k = p.k; tp.ldc = p.ldc; tp.epi = p.epi; tp.bf16 = bf16 ? 1 : 0;
     if (p.epi == GEMM_EPI_ROPE_SPLIT) tp.rope = *p.rope;
     // persistent grid: one CTA per SM walks the tiles, M tiles fastest (the CTAs that share a weight tile run together)
-    static const int n_sm = []() { int dev = 0, n = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); return n > 0 ? n : 148; }();
-    static const bool persist = []() { const char* e = getenv("GL_TC5_PERSIST"); return !(e && e[0] == '0'); }();
-    // tile width: 128 x 256 tiles stage 25 % fewer bytes per MAC (the L2 -> shared-memory feed is the limit of this kernel);
-    // taken when they do not cost whole waves of the persistent grid (GL_TC5_BN = 128 / 256 forces one for A/B runs)
-    static const int force_bn = []() { const char* e = getenv("GL_TC5_BN"); return e ? atoi(e) : 0; }();
-    const int tiles_m = (p.m + BM - 1) / BM;
-    const int t128 = tiles_m * ((p.n + 127) / 128), t256 = tiles_m * ((p.n + 255) / 256);
-    auto waves = [&](int t) { return (t + n_sm - 1) / n_sm; };
-    bool wide = p.m > 128 && p.n >= 512 && 2 * waves(t256) <= waves(t128) + (waves(t128) > 6 ? 1 : 0);
-    if (force_bn == 128) wide = false;
-    if (force_bn == 256) wide = p.n >= 256;
-    // CTA pairs (cta_group::2, 256 x 256 tiles on two SMs) where they do not cost whole waves: time in units of one 128 x 128 tile
-    // on one SM.  GL_TC5_PAIR = 0 never, 1 (default) by this rule, 2 whenever the shape allows it (tests, A/B runs).
-    const int pair_mode = []() { const char* e = getenv("GL_TC5_PAIR"); return e ? atoi(e) : 1; }();      // read per launch: tests flip it inside one process
-    const int t_pair = ((p.m + 255) / 256) * ((p.n + 255) / 256);
-    const int cost_single = wide ? 2 * waves(t256) : waves(t128);
-    const int cost_pair = 2 * ((t_pair + n_sm / 2 - 1) / (n_sm / 2));
-    if (p.m > 128 && p.n >= 256 && (pair_mode == 2 || (pair_mode == 1 && cost_pair <= cost_single))) {
-        cudaLaunchConfig_t cfg{};
-        cfg.blockDim = dim3(TC5_THREADS);
-        cfg.dynamicSmemBytes = Tc5Cfg<256, 2>::SMEM;
-        cfg.stream = s;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        cfg.attrs = at;
-        cfg.numAttrs = 1;
-        // pairs that can be resident at once (one per TPC unless the device says otherwise): the persistent grid is that wide
-        static const int max_pairs = [&]() {
-            cudaLaunchConfig_t q = cfg;
-            q.gridDim = dim3((unsigned)(2 * (n_sm / 2)));
-            int n = 0;
-            if (cudaOccupancyMaxActiveClusters(&n, gemm_tc5_kernel<256, 2>, &q) != cudaSuccess || n < 1) { cudaGetLastError(); n = n_sm / 2; }
-            return std::min(n, n_sm / 2);
-        }();
-        const int pairs = std::max(1, std::min(t_pair, max_pairs));
-        cfg.gridDim = dim3((unsigned)(2 * pairs));
-        return cudaLaunchKernelEx(&cfg, gemm_tc5_kernel<256, 2>, tp);
-    }
-    if (wide) {
-        const dim3 grid((unsigned)(persist ? std::min(t256, n_sm) : t256));
-        gemm_tc5_kernel<256, 1><<<grid, TC5_THREADS, Tc5Cfg<256, 1>::SMEM, s>>>(tp);
-    } else {
-        const dim3 grid((unsigned)(persist ? std::min(t128, n_sm) : t128));
-        gemm_tc5_kernel<128, 1><<<grid, TC5_THREADS, Tc5Cfg<128, 1>::SMEM, s>>>(tp);
-    }
+    static const int n_sm = []() { int dev = 0, n = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); return n > 0 ? n : 132; }();
+    const int tiles = ((p.m + BM - 1) / BM) * ((p.n + BN - 1) / BN);
+    const dim3 grid((unsigned)std::min(tiles, n_sm));
+    if (bf16) gemm_tc5_kernel<true><<<grid, TC_THREADS, TC_SMEM, s>>>(tp);
+    else gemm_tc5_kernel<false><<<grid, TC_THREADS, TC_SMEM, s>>>(tp);
     return cudaGetLastError();
 }
 

@@ -6,31 +6,29 @@
 // more than one job (WorkerClientService.ts:500-505; MAX_CONCURRENT_JOBS_PER_WORKER, server/src/config/index.ts:31).
 //
 // Bound: HBM.  A step streams the model's 4.6 GB once; at B = 32 the tensor work is 128 x 32 x 64 MACs per 16 KB of weights
-// (16 cycles of tcgen05 against ~800 cycles of HBM time per qtile and SM), so the tensor pipe idles and the CUDA cores'
+// (a few dozen tensor-core cycles against ~1 000 cycles of HBM time per qtile and SM), so the tensor pipe idles and the CUDA cores'
 // job -- ~2.3 lane-operations per weight to unpack nibbles into fp16 -- is what has to keep up with the memory pipe.
 //
-// Shape of the kernel (persistent, one CTA per SM, 24 warps, hand-written PTX; layouts and the per-thread unpack program in
+// Shape of the kernel (persistent, one CTA per SM, 16 warps, hand-written PTX; layouts and the per-thread unpack program in
 // qgemm_layout.h, which the CPU suite runs bit for bit):
 //   the weights of a GEMM are a stream of QTILES (128 rows x 256 columns, one contiguous 18 / 26 KB range each); the U = tiles x
 //   K-blocks qtiles are dealt to the G CTAs as contiguous ranges [c U / G, (c+1) U / G) ("stream-K": perfect balance for every
-//   shape -- 32 tiles x 16 blocks on 148 SMs as well as 1002 x 16 -- and every CTA streams ONE contiguous byte range);
-//   warp 0 / one lane : weight producer -- per qtile one 1-D TMA bulk copy of the raw bytes into a 6-8 stage ring (all the
-//                       shared memory the activations leave: 110-190 KB in flight per SM);
-//   warp 2 / one lane : activation producer -- four 2-D TMA boxes [B x 64] fp16 per qtile (L2-resident), two qtiles deep;
-//   warps 4..19       : unpack -- thread (row, K-step) turns 64 columns of its row into 32 packed half2 REGISTERS and writes them
-//                       with one tcgen05.st.32x32b.x32 into TENSOR MEMORY: the A operand [128 lanes x 32 columns] of that K-step
-//                       (ring of 8 K-steps = 256 TMEM columns).  The dequantised weights never touch shared memory: the only
-//                       shared-memory traffic per qtile is the raw bytes (in, out) and the activations;
-//   warp 1 / one lane : MMA issuer -- per K-step four tcgen05.mma.cta_group::1.kind::f16 with A FROM TMEM and B = the activation
-//                       box in shared memory (M 128 = weight rows, N = B, K 16), accumulator [128 lanes x B columns] fp32 in
-//                       TMEM, double-buffered across output tiles; tcgen05.commit hands K-step slots / boxes / accumulators on;
-//   warps 20..23      : epilogue -- tcgen05.ld 16 batch columns at a time, then the fused epilogue (fp32 store, residual add,
-//                       SiLU*mul -> fp16).  An output tile whose K range is shared with neighbouring CTAs is finished by the
-//                       lowest-numbered of them (its part of the tile is the END of its range, the others' the START of theirs):
-//                       the others store their partial to scratch and count themselves in, the finisher adds the partials IN
-//                       CTA ORDER (deterministic) to its accumulator and runs the epilogue.
-// SASS to look for: UTCHMMA (tcgen05.mma), STTM (tcgen05.st), LDTM (tcgen05.ld), UBLKCP (1-D bulk copy), UTMALDG (2-D TMA),
-// UTCBAR (commit).
+//   shape -- 32 tiles x 16 blocks on 132 SMs as well as 1002 x 16 -- and every CTA streams ONE contiguous byte range);
+//   warp 0 / one lane : weight producer -- per qtile one 1-D TMA bulk copy of the raw bytes into a 2-8 stage ring (the shared
+//                       memory the operands leave);
+//   warp 1 / one lane : activation producer -- four 2-D TMA boxes [B x 64] fp16 per qtile (L2-resident);
+//   warps 4..11       : unpack -- thread (row, half) turns 128 columns of its row into 2 x 32 packed half2 registers and stores
+//                       them into the A operand of the qtile in shared memory (four K-steps [128 rows x 64] fp16, 128-byte
+//                       swizzle); the next qtile's first K-step is unpacked into registers while the MMAs of this one run;
+//   warps 12..15      : one warpgroup: MMA and epilogue -- per qtile 32 wgmma.m64nBk16 (two 64-row halves x 16 K-steps of 16,
+//                       A and B from shared memory, fp32 accumulator in registers); after the last qtile of an output tile the
+//                       accumulator is staged in the consumed A operand (row-contiguous per batch column) and each thread runs
+//                       the fused epilogue of one weight row (fp32 store, residual add, SiLU*mul -> fp16).  An output tile
+//                       whose K range is shared with neighbouring CTAs is finished by the lowest-numbered of them (its part of
+//                       the tile is the END of its range, the others' the START of theirs): the others store their partial to
+//                       scratch and count themselves in, the finisher adds the partials IN CTA ORDER (deterministic) to its
+//                       accumulator and runs the epilogue.
+// SASS to look for: HGMMA (wgmma), UBLKCP (1-D bulk copy), UTMALDG (2-D TMA).
 #include <cuda.h>
 #include <algorithm>
 #include <cstdlib>
@@ -40,24 +38,25 @@
 #include "common.cuh"
 #include "qgemm.h"
 #include "qgemm_layout.h"
+#include "wgmma.cuh"
 
 namespace gl {
 
 namespace {
 
-constexpr int QG_THREADS = 24 * 32;
-constexpr int QG_W_UNPACK0 = 4, QG_N_UNPACK = 16, QG_W_EPI0 = 20;
-constexpr int QG_A_UNITS = 2;                        // operand ring: the A operand (TMEM, 4 K-steps x 32 columns) and the activation boxes (shared memory) of two qtiles
-constexpr int QG_A_COL0 = 128;                       // TMEM columns [0, 128): two accumulators of up to 64; [128, 384): the A ring
-constexpr int QG_TMEM_COLS = 512;                    // power of two >= 384 (one CTA per SM: nobody else wants the rest)
-constexpr size_t QG_SMEM = 227 * 1024;               // the whole opt-in shared memory; the raw ring takes what the activations leave
+constexpr int QG_THREADS = 16 * 32;
+constexpr int QG_W_UNPACK0 = 4, QG_N_UNPACK = 8, QG_W_EPI0 = 12;    // the MMA / epilogue warps are one warpgroup (warp index % 4 == 0)
+constexpr int QG_A_BYTES = 4 * QG_ROWS * QG_KSTEP * 2;               // the A operand of one qtile: four K-steps [128 x 64] fp16 (64 KB)
+constexpr int QG_STG_LD = QG_ROWS + 4;                               // accumulator staging: [NB][132] fp32, row-contiguous per batch column
+constexpr size_t QG_SMEM = 227 * 1024;               // the whole opt-in shared memory; the raw ring takes what the operands leave
 
 template <int NB> struct QCfg {
     static constexpr int B_TILE = NB * 128;          // activations [NB rows x 64] fp16, 128-byte swizzle
-    static constexpr int ACT_BYTES = QG_A_UNITS * 4 * B_TILE;
-    static constexpr int BAR_BYTES = 1536;         // mbarriers, TMEM address, folded-RMSNorm scratch (64 + 128 floats)
+    static constexpr int ACT_BYTES = 4 * B_TILE;
+    static constexpr int BAR_BYTES = 1536;         // mbarriers, folded-RMSNorm scratch (64 + 128 floats)
     static constexpr int CK_BYTES = 2 * 4 * NB * 32 * 4;       // cluster mode: two rounds x four source ranks x [NB columns][32 rows] fp32
-    static constexpr int RAW_BUDGET = (int)QG_SMEM - 1024 /* alignment */ - BAR_BYTES - ACT_BYTES;
+    static constexpr int RAW_BUDGET = (int)QG_SMEM - 1024 /* alignment */ - BAR_BYTES - ACT_BYTES - QG_A_BYTES;
+    static_assert(NB * QG_STG_LD * 4 <= QG_A_BYTES, "the accumulator staging lives in the A operand");
 };
 constexpr int QG_MAX_RAW_STAGES = 8;
 
@@ -94,63 +93,6 @@ __device__ __forceinline__ void tma_load_2d_q(void* dst, const CUtensorMap* map,
                  "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
                  : "memory");
 }
-__device__ __forceinline__ bool q_elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P1;\n\telect.sync _|P1, 0xffffffff;\n\tselp.b32 %0, 1, 0, P1;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void q_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void q_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void q_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[tmem: 128 lanes x 8 columns of two fp16] x B[smem descriptor]: the ".ts" form of the instruction
-__device__ __forceinline__ void q_mma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// 32 lanes x 32 columns: thread t of the warp writes its 32 registers to columns [col, col + 32) of lane (lane base + t)
-__device__ __forceinline__ void tmem_st_32x32_nowait(uint32_t taddr, const uint32_t* w) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, "
-        "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]), "r"(w[8]), "r"(w[9]), "r"(w[10]),
-          "r"(w[11]), "r"(w[12]), "r"(w[13]), "r"(w[14]), "r"(w[15]), "r"(w[16]), "r"(w[17]), "r"(w[18]), "r"(w[19]), "r"(w[20]), "r"(w[21]),
-          "r"(w[22]), "r"(w[23]), "r"(w[24]), "r"(w[25]), "r"(w[26]), "r"(w[27]), "r"(w[28]), "r"(w[29]), "r"(w[30]), "r"(w[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t* w) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, "
-        "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]), "r"(w[8]), "r"(w[9]), "r"(w[10]),
-          "r"(w[11]), "r"(w[12]), "r"(w[13]), "r"(w[14]), "r"(w[15]), "r"(w[16]), "r"(w[17]), "r"(w[18]), "r"(w[19]), "r"(w[20]), "r"(w[21]),
-          "r"(w[22]), "r"(w[23]), "r"(w[24]), "r"(w[25]), "r"(w[26]), "r"(w[27]), "r"(w[28]), "r"(w[29]), "r"(w[30]), "r"(w[31])
-        : "memory");
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-// K-major operand tile, 128-byte swizzle, rows of 64 fp16 (8-row atoms of 1024 B): the descriptor prefill_tc5.cu uses
-__device__ __forceinline__ uint64_t q_desc_sw128(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-// 32 lanes x 16 columns of fp32: thread t of the warp receives row (lane base + t), 16 consecutive columns
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, float* v) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
 // the range of qtile units CTA c owns, and who shares an output tile with whom
 __device__ __forceinline__ long long q_range_start(int c, long long U, int G) { return (long long)c * U / G; }
 // largest c with range_start(c) <= x
@@ -254,25 +196,24 @@ __global__ void __launch_bounds__(QG_THREADS, 1) qgemm_kernel(const __grid_const
     using Cfg = QCfg<NB>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t* act_ring = smem;                                                 // [2][4][NB x 64 fp16]      TMA (L2)     -> tensor core
-    float* recv = reinterpret_cast<float*>(act_ring + Cfg::ACT_BYTES);        // cluster mode: [2 rounds][4 ranks][NB][32 rows] partial slices
-    uint8_t* raw_ring = act_ring + Cfg::ACT_BYTES + (p.ck_s ? Cfg::CK_BYTES : 0);   // [raw_stages][raw_stride]  TMA (HBM) -> unpack warps
+    uint8_t* act_ring = smem;                                                 // [4][NB x 64 fp16]          TMA (L2)      -> tensor core
+    uint8_t* a_op = act_ring + Cfg::ACT_BYTES;                                // [4][128 x 64 fp16]         unpack warps  -> tensor core
+    float* stg = reinterpret_cast<float*>(a_op);                              // [NB][QG_STG_LD] fp32       accumulator staging (A consumed)
+    float* recv = reinterpret_cast<float*>(a_op + QG_A_BYTES);                // cluster mode: [2 rounds][4 ranks][NB][32 rows] partial slices
+    uint8_t* raw_ring = a_op + QG_A_BYTES + (p.ck_s ? Cfg::CK_BYTES : 0);     // [raw_stages][raw_stride]  TMA (HBM)     -> unpack warps
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (QG_SMEM - 1024 - Cfg::BAR_BYTES));
     uint64_t* raw_full = bars;                               // [8]  producer (tx bytes)                     -> unpack warps
-    uint64_t* raw_empty = raw_full + QG_MAX_RAW_STAGES;      // [8]  8 unpack warps (one group)             -> producer
-    uint64_t* unit_full = raw_empty + QG_MAX_RAW_STAGES;     // [2]  8 unpack warps + activations (tx bytes)  -> MMA issuer
-    uint64_t* unit_empty = unit_full + QG_A_UNITS;           // [2]  commit                                  -> unpack warps, activation producer
-    uint64_t* acc_full = unit_empty + QG_A_UNITS;            // [2]  commit                                  -> epilogue
-    uint64_t* acc_empty = acc_full + 2;                      // [2]  4 epilogue warps                        -> MMA issuer
-    uint64_t* recv_bar = acc_empty + 2;                      // [2]  cluster mode: 4 ranks' epilogue warps    -> this rank's epilogue
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(recv_bar + 2);
-    float* inv_s = reinterpret_cast<float*>(tmem_slot + 2);  // [64] folded RMSNorm: 16 / rms of every token of the step
+    uint64_t* raw_empty = raw_full + QG_MAX_RAW_STAGES;      // [8]  the unpack warps                        -> producer
+    uint64_t* unit_full = raw_empty + QG_MAX_RAW_STAGES;     // [1]  unpack warps + activations (tx bytes)   -> MMA warpgroup
+    uint64_t* unit_empty = unit_full + 1;                    // [1]  MMA warpgroup                           -> unpack warps, activation producer
+    uint64_t* recv_bar = unit_empty + 1;                     // [2]  cluster mode: 4 ranks' epilogue warps    -> this rank's epilogue
+    float* inv_s = reinterpret_cast<float*>(recv_bar + 2);   // [64] folded RMSNorm: 16 / rms of every token of the step
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int G = gridDim.x, cta = blockIdx.x;
     const int nkb = p.nkb;
     if (threadIdx.x == 0) q_stamp(p, 0);                                      // CTA entry
-    const int U = p.n_tiles * nkb;                                            // < 2^31 / 148 for every matrix of these models
+    const int U = p.n_tiles * nkb;                                            // < 2^31 / 132 for every matrix of these models
     const bool ck = p.ck_s != 0;
     const int rank = ck ? (int)q_cluster_rank() : 0, cluster = cta / QG_CK;
     QWalk wk;
@@ -289,29 +230,23 @@ __global__ void __launch_bounds__(QG_THREADS, 1) qgemm_kernel(const __grid_const
     }
     const int R = p.raw_stages;
 
-    if (warp == 2 && lane == 0) asm volatile("prefetch.tensormap [%0];" ::"l"(&p.tb) : "memory");
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < QG_MAX_RAW_STAGES; ++i) { mbar_init(&raw_full[i], 1); mbar_init(&raw_empty[i], QG_N_UNPACK / 2); }
-        for (int i = 0; i < QG_A_UNITS; ++i) { mbar_init(&unit_full[i], QG_N_UNPACK / 2 + 1); mbar_init(&unit_empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 4); mbar_init(&recv_bar[i], QG_CK); }
+    if (warp == 1 && lane == 0) asm volatile("prefetch.tensormap [%0];" ::"l"(&p.tb) : "memory");
+    if (warp == 0 && lane == 0) {
+        for (int i = 0; i < QG_MAX_RAW_STAGES; ++i) { mbar_init(&raw_full[i], 1); mbar_init(&raw_empty[i], QG_N_UNPACK); }
+        mbar_init(&unit_full[0], QG_N_UNPACK + 1);
+        mbar_init(&unit_empty[0], 1);
+        for (int i = 0; i < 2; ++i) mbar_init(&recv_bar[i], QG_CK);
         fence_mbar_init();
     }
-    if (warp == 3) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(QG_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    q_fence_before();
     __syncthreads();
-    q_fence_after();
     if (ck) {       // nobody may arrive on a peer's barrier before that peer has initialised it
         asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
         asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
     }
-    const uint32_t tmem_base = *tmem_slot;
-    if (threadIdx.x == 0) q_stamp(p, 1);                                      // barriers, tensor memory ready
+    if (threadIdx.x == 0) q_stamp(p, 1);                                      // barriers ready
 
-    // Programmatic dependent launch: everything up to here, the weight stream and the unpacking of the first two qtiles need
-    // nothing from the kernel before -- only the activations (read) and C / the split-tile scratch (written) do.
+    // Programmatic dependent launch: everything up to here, the weight stream and the unpacking of the first qtile need nothing
+    // from the kernel before -- only the activations (read) and C / the split-tile scratch (written) do.
     pdl_launch_dependents();
     if (warp == 0) {
         if (lane == 0) {
@@ -333,107 +268,122 @@ __global__ void __launch_bounds__(QG_THREADS, 1) qgemm_kernel(const __grid_const
                 wk.advance(tile, kb, 1);
             }
         }
-    } else if (warp == 2) {
+    } else if (warp == 1) {
         if (lane == 0) {
-            // ===== activation producer: the four [NB x 64] boxes of a qtile's K range (L2-resident), two qtiles deep =====
+            // ===== activation producer: the four [NB x 64] boxes of a qtile's K range (L2-resident) =====
             int tile = wk.tile0, kb = wk.kb0;
             pdl_wait();                                               // the activations are the output of the kernel before
             q_stamp(p, 8);                                                    // the kernel before has completed
             for (int i = 0; i < wk.n; ++i) {
-                const int s = i & 1;
-                uint8_t* st = act_ring + (size_t)s * 4 * Cfg::B_TILE;
-                mbar_wait(&unit_empty[s], ((uint32_t)(i >> 1) & 1u) ^ 1u);
-                mbar_expect_tx(&unit_full[s], 4u * Cfg::B_TILE);
+                mbar_wait(&unit_empty[0], (uint32_t)(i & 1) ^ 1u);
+                mbar_expect_tx(&unit_full[0], 4u * Cfg::B_TILE);
 #pragma unroll
-                for (int kk = 0; kk < 4; ++kk) tma_load_2d_q(st + kk * Cfg::B_TILE, &p.tb, kb * QG_COLS + kk * QG_KSTEP, 0, &unit_full[s]);
+                for (int kk = 0; kk < 4; ++kk) tma_load_2d_q(act_ring + kk * Cfg::B_TILE, &p.tb, kb * QG_COLS + kk * QG_KSTEP, 0, &unit_full[0]);
                 wk.advance(tile, kb, 1);
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        // The WHOLE warp walks the loop with warp-uniform values and one elected lane issues: written as `if (lane == 0) { ... }`
-        // the compiler cannot keep the operands in uniform registers and wraps every tcgen05 instruction in a convert-to-uniform
-        // loop (ELECT / 4 x R2UR / UTCHMMA / BRA.U.ANY: ~15 dependent instructions per MMA).  One thread then needed ~4 000 cycles for
-        // the 16 MMAs, 5 commits and 5 waits of a qtile -- and that, not HBM or the unpack warps, set the pace of the kernel
-        // (profiles/r02_qgemm_notes.md).  One wait, 16 MMAs and one commit per qtile now.
-        // instruction descriptor: D = F32, A / B = F16, both K-major, N = NB, M = 128
-        const uint32_t idesc = (1u << 4) | ((uint32_t)(NB >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        const uint32_t tb = __shfl_sync(0xffffffffu, tmem_base, 0);
-        const uint32_t act_u32 = __shfl_sync(0xffffffffu, smem_u32(act_ring), 0);
-        int seg = 0, kb = wk.kb0;
-        for (int i = 0; i < wk.n; ++seg) {
-            const int n_kb = min(wk.kb_end - kb, wk.n - i);
-            kb = wk.kb_begin;
-            const int buf = seg & 1;
-            mbar_wait(&acc_empty[buf], ((uint32_t)(seg >> 1) & 1u) ^ 1u);
-            const uint32_t tmem_d = tb + (uint32_t)(buf * NB);
-            for (int j = 0; j < n_kb; ++j, ++i) {
-                const int sa = i & 1;
-                mbar_wait(&unit_full[sa], (uint32_t)(i >> 1) & 1u);   // A operand in TMEM (one unpack group) and activation boxes (TMA) are there
-                q_fence_after();
-                const uint32_t ta = tb + (uint32_t)(QG_A_COL0 + sa * 128);
-                const uint64_t bdesc = q_desc_sw128(act_u32 + (uint32_t)(sa * 4 * Cfg::B_TILE));
-                if (q_elect_one()) {
-#pragma unroll
-                    for (int kk = 0; kk < 4; ++kk)
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)                   // K = 16 per instruction: 8 TMEM columns of A, 32 bytes of B
-                            q_mma_f16_ts(tmem_d, ta + (uint32_t)(kk * 32 + k * 8), bdesc + (uint64_t)(kk * (Cfg::B_TILE >> 4) + 2 * k), idesc,
-                                         (kk | k) ? 1u : (j ? 1u : 0u));
-                    q_commit(&unit_empty[sa]);                        // TMEM slot and activation boxes may be overwritten once these MMAs are done
-                    if (j == n_kb - 1) q_commit(&acc_full[buf]);
-                }
-                __syncwarp();
-            }
-        }
-        if (lane == 0) q_stamp(p, 9);                                         // last MMA issued
     } else if (warp >= QG_W_UNPACK0 && warp < QG_W_EPI0) {
-        // ===== unpack warps: two groups of eight; group g owns the qtiles i = g (mod 2) of the CTA's sequence and slot g of the
-        // operand ring.  Thread (row r, half h) of a group turns 128 columns of its row into two K-steps (2 x 32 registers, two
-        // tcgen05.st).  Two qtiles are therefore in flight at once, and a warp pays the fixed latencies of an iteration (barrier
-        // polls, tcgen05.wait::st, arrive -> MMA -> commit round trip) once per 128 columns.  The warp's TMEM lane quarter
-        // (warp % 4) is r / 32.
-        const int t = (warp - QG_W_UNPACK0) * 32 + lane, grp = t >> 8, r = t & 127, h = (t >> 7) & 1;
-        const uint32_t ta0 = tmem_base + ((uint32_t)(r & ~31) << 16) + (uint32_t)(QG_A_COL0 + grp * 128 + h * 64);
-        int tile = wk.tile0, kb = wk.kb0, s = grp % R, cur = -1, type = 12;
-        if (grp) wk.advance(tile, kb, 1);
-        uint32_t ph = (uint32_t)(grp / R) & 1u, n = 0;
-        for (int i = grp; i < wk.n; i += 2, ++n) {
+        // ===== unpack warps: thread (row r, half h) turns 128 columns of its row into two K-steps (2 x 32 registers) and stores
+        // them into the A operand: row r of K-step kk at kk * 16 KB + 128 r, 16-byte chunk c at position c ^ (r % 8) (the 128-byte
+        // swizzle the MMA's descriptor names; the eight rows of a quarter-warp store to eight different bank groups).
+        const int t = (warp - QG_W_UNPACK0) * 32 + lane, r = t & 127, h = t >> 7;
+        uint8_t* arow = a_op + (size_t)r * 128;
+        auto store = [&](int kk, const uint32_t* w) {
+#pragma unroll
+            for (int c = 0; c < 8; ++c)
+                *reinterpret_cast<uint4*>(arow + kk * (QG_ROWS * QG_KSTEP * 2) + ((c ^ (r & 7)) << 4)) = make_uint4(w[4 * c], w[4 * c + 1], w[4 * c + 2], w[4 * c + 3]);
+        };
+        int tile = wk.tile0, kb = wk.kb0, s = 0, cur = -1, type = 12;
+        uint32_t ph = 0;
+        for (int i = 0; i < wk.n; ++i) {
             if (tile != cur) { cur = tile; type = q_tile_type(p, tile); }
             const uint8_t* raw = raw_ring + (size_t)s * p.raw_stride;
             mbar_wait(&raw_full[s], ph);
-            if (n == 0 && t == 0) q_stamp(p, 3);                              // first qtile has landed
+            if (i == 0 && t == 0) q_stamp(p, 3);                              // first qtile has landed
             uint32_t w[32];
             qg_dequant_kstep(type, raw, r, 2 * h, [&](int c, QgU4 v) { w[4 * c] = v.x; w[4 * c + 1] = v.y; w[4 * c + 2] = v.z; w[4 * c + 3] = v.w; });
-            // the first 32 words sit in registers: only now does the thread need its TMEM slot (the MMAs of this group's previous
-            // qtile are done)
-            mbar_wait(&unit_empty[grp], (n & 1u) ^ 1u);
-            q_fence_after();
-            tmem_st_32x32_nowait(ta0, w);
+            // the first 32 words sit in registers: only now does the thread need the A operand (the MMAs of the previous qtile
+            // are done and its accumulator staging has been read)
+            mbar_wait(&unit_empty[0], (uint32_t)(i & 1) ^ 1u);
+            store(2 * h, w);
             qg_dequant_kstep(type, raw, r, 2 * h + 1, [&](int c, QgU4 v) { w[4 * c] = v.x; w[4 * c + 1] = v.y; w[4 * c + 2] = v.z; w[4 * c + 3] = v.w; });
             __syncwarp();
             if (lane == 0) mbar_arrive(&raw_empty[s]);                // this warp has read all it needs of the raw bytes
-            tmem_st_32x32_nowait(ta0 + 32, w);
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            q_fence_before();
+            store(2 * h + 1, w);
+            fence_proxy_async();                                      // generic-proxy stores -> the tensor core's (async-proxy) reads
             __syncwarp();
-            if (lane == 0) mbar_arrive(&unit_full[grp]);
-            s += 2;
-            if (s >= R) { s -= R; ph ^= 1u; }
-            wk.advance(tile, kb, 2);
+            if (lane == 0) mbar_arrive(&unit_full[0]);
+            if (++s == R) { s = 0; ph ^= 1u; }
+            wk.advance(tile, kb, 1);
         }
-        if ((t & 255) == 0) q_stamp(p, 4 + grp);                              // this group has unpacked its last qtile
+        if (t == 0) q_stamp(p, 4);                                            // the last qtile is unpacked
     } else if (warp >= QG_W_EPI0) {
-        // ===== epilogue warps =====
-        const int q = warp & 3;                                       // TMEM lane quarter this warp may access
+        // ===== MMA and epilogue warpgroup =====
+        const int q = warp & 3;                                       // rows 32q..32q+31 of the tile in the epilogue
         const int nl = q * 32 + lane;                                 // row inside the tile
+        const int et = threadIdx.x - QG_W_EPI0 * 32;
         int seg = 0, tile = wk.tile0, kb = wk.kb0;
+        const uint32_t act_u32 = smem_u32(act_ring), a_u32 = smem_u32(a_op);
+        // the MMAs of qtiles [i0, i0 + n_kb) (one output tile) into the registers, then the accumulator into the staging rows: after
+        // this stg[b * QG_STG_LD + row] = C[b][row] of the CTA's part of the tile; the A operand stays claimed until release()
+        auto mma_segment = [&](int i0, int n_kb) {
+            float acc[2][NB / 2];
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+                for (int x = 0; x < NB / 2; ++x) acc[hf][x] = 0.f;
+            for (int j = 0; j < n_kb; ++j) {
+                const int i = i0 + j;
+                mbar_wait(&unit_full[0], (uint32_t)(i & 1));          // A operand (unpack warps) and activation boxes (TMA) are there
+                wgmma_fence_acc<NB / 2>(acc[0]);
+                wgmma_fence_acc<NB / 2>(acc[1]);
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) {
+                    const uint64_t bdesc = wgmma_desc_sw128(act_u32 + (uint32_t)(kk * Cfg::B_TILE));
+#pragma unroll
+                    for (int hf = 0; hf < 2; ++hf) {
+                        const uint64_t adesc = wgmma_desc_sw128(a_u32 + (uint32_t)(kk * (QG_ROWS * QG_KSTEP * 2) + hf * (64 * QG_KSTEP * 2)));
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) wgmma_m64k16<NB, false>(acc[hf], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), 1u);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_acc<NB / 2>(acc[0]);
+                wgmma_fence_acc<NB / 2>(acc[1]);
+                if (j < n_kb - 1) {
+                    named_bar_sync(1, 128);                           // every thread's MMAs of this qtile are complete
+                    if (et == 0) mbar_arrive(&unit_empty[0]);
+                }
+            }
+            if (i0 + n_kb >= wk.n && et == 0) q_stamp(p, 9);          // last MMA complete
+            named_bar_sync(1, 128);
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+                for (int x = 0; x < NB / 8; ++x) {
+                    const int row = hf * 64 + q * 16 + (lane >> 2), b = 8 * x + 2 * (lane & 3);
+                    stg[b * QG_STG_LD + row] = acc[hf][4 * x];
+                    stg[(b + 1) * QG_STG_LD + row] = acc[hf][4 * x + 1];
+                    stg[b * QG_STG_LD + row + 8] = acc[hf][4 * x + 2];
+                    stg[(b + 1) * QG_STG_LD + row + 8] = acc[hf][4 * x + 3];
+                }
+            named_bar_sync(1, 128);
+        };
+        auto staged16 = [&](int c, float* v) {
+#pragma unroll
+            for (int b = 0; b < 16; ++b) v[b] = stg[(c * 16 + b) * QG_STG_LD + nl];
+        };
+        auto release = [&]() {                                        // the staging has been read: the A operand may be refilled
+            named_bar_sync(1, 128);
+            if (et == 0) mbar_arrive(&unit_empty[0]);
+        };
         pdl_wait();                                                   // C, the scratch and the tickets may still be in use by the kernel before
         const float* inv = nullptr;
         if (p.ssq_in != nullptr) {
             // folded RMSNorm, consumer side: token b's sum of squares = the parts the GEMM before wrote, added in part order by ONE
             // thread per token (every CTA computes the same 64 numbers; the loads hit L2 and hide behind the first qtiles)
-            const int et = threadIdx.x - QG_W_EPI0 * 32;
             constexpr int GROUPS = 128 / NB;                          // threads per token: each sums every GROUPS-th part
             const int b = et % NB, g = et / NB;
             float acc = 0.f;
@@ -460,8 +410,8 @@ __global__ void __launch_bounds__(QG_THREADS, 1) qgemm_kernel(const __grid_const
         for (int i = 0; i < wk.n; ++seg, tile += wk.tile_step) {
             const int n_kb = min(wk.kb_end - kb, wk.n - i);
             kb = wk.kb_begin;
+            const int i0 = i;
             i += n_kb;
-            const int buf = seg & 1;
             if (ck) {
                 // ---- cluster mode: this CTA's accumulator is one K-quarter of the tile.  Warp q holds rows 32q..32q+31 of it: they
                 // belong to the slice rank q finishes, so the warp stores them straight into rank q's shared memory (slot = own rank)
@@ -478,22 +428,17 @@ __global__ void __launch_bounds__(QG_THREADS, 1) qgemm_kernel(const __grid_const
 #pragma unroll
                     for (int b = 0; b < CPT; ++b) old[b] = n < p.n ? __ldcg(reinterpret_cast<const float*>(p.c) + (size_t)(q * CPT + b) * p.ldc + n) : 0.f;
                 }
-                mbar_wait(&acc_full[buf], (uint32_t)(seg >> 1) & 1u);
-                q_fence_after();
+                mma_segment(i0, n_kb);
                 if (i >= wk.n && warp == QG_W_EPI0 && lane == 0) q_stamp(p, 6);
                 const uint32_t dst = q_mapa(smem_u32(recv + (size_t)(par * QG_CK + rank) * SLOT), (uint32_t)q) + (uint32_t)lane * 4u;
 #pragma unroll
                 for (int c = 0; c < NB / 16; ++c) {
                     float v[16];
-                    tmem_ld_32x16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * NB + c * 16), v);
-                    if (c == NB / 16 - 1) {
-                        q_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(&acc_empty[buf]);
-                    }
+                    staged16(c, v);
 #pragma unroll
                     for (int b = 0; b < 16; ++b) q_st_cluster_f32(dst + (uint32_t)((c * 16 + b) * 32 * 4), v[b]);
                 }
+                release();
                 __syncwarp();
                 if (lane == 0) q_arrive_cluster(q_mapa(smem_u32(&recv_bar[par]), (uint32_t)q));
                 q_wait_cluster(&recv_bar[par], (uint32_t)(seg >> 1) & 1u);
@@ -533,18 +478,15 @@ __global__ void __launch_bounds__(QG_THREADS, 1) qgemm_kernel(const __grid_const
             // Shared tile.  Its FIRST units are the END of CTA c_first's range, its later units the START of the ranges of
             // c_first + 1 .. c_last: those CTAs store their part to scratch and count themselves in; c_first gets there last (or
             // together with the CTAs whose whole range lies inside the tile), so it is the designated finisher -- it keeps its own
-            // part in tensor memory, adds the others' (CTA order: deterministic) and runs the epilogue.  It polls the counter and
-            // fetches the partials while its own MMAs are still running.  (All CTAs of the grid are resident -- one per SM -- and
-            // nobody waits for a lower-numbered CTA, so the wait cannot deadlock.)  Two alternatives were measured and dropped:
-            // "last to arrive finishes" (ticket; the finisher then starts the exchange only after its own part: +4 us per launch,
-            // run L) and "all K contributors finish a slice each" (two shared tiles per CTA, each a chain of five global round trips
-            // at the very end: +6 us, run N).
+            // part in registers, adds the others' (CTA order: deterministic) and runs the epilogue.  (All CTAs of the grid are
+            // resident -- one per SM -- and nobody waits for a lower-numbered CTA, so the wait cannot deadlock.)
             const int t0 = tile * nkb;
             const int c_first = whole ? cta : q_owner_of(t0, U, G), c_last = whole ? cta : q_owner_of(t0 + nkb - 1, U, G);
             const bool finisher = !whole && cta == c_first;
             float* mine = p.partial + (size_t)cta * (NB * QG_ROWS) + nl;
             constexpr bool PRE = NB <= 32;                            // the others' sum fits the registers beside the accumulator chunk
             float ps[PRE ? NB : 1];
+            mma_segment(i0, n_kb);
             if (finisher) {
                 if (warp == QG_W_EPI0 && lane == 0) {
                     const unsigned need = (unsigned)(c_last - c_first);
@@ -570,18 +512,11 @@ __global__ void __launch_bounds__(QG_THREADS, 1) qgemm_kernel(const __grid_const
                     }
                 }
             }
-            mbar_wait(&acc_full[buf], (uint32_t)(seg >> 1) & 1u);
-            q_fence_after();
             if (i >= wk.n && warp == QG_W_EPI0 && lane == 0) q_stamp(p, 6);   // last accumulator complete
 #pragma unroll
             for (int c = 0; c < NB / 16; ++c) {
                 float v[16];
-                tmem_ld_32x16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * NB + c * 16), v);
-                if (c == NB / 16 - 1) {
-                    q_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&acc_empty[buf]);      // the accumulator has been read: the tile after next may start
-                }
+                staged16(c, v);
                 if (whole) q_epilogue16(p, n, lane, c * 16, v, inv);
                 else if (finisher) {
                     if (PRE) {
@@ -603,6 +538,7 @@ __global__ void __launch_bounds__(QG_THREADS, 1) qgemm_kernel(const __grid_const
                     for (int b = 0; b < 16; ++b) mine[(c * 16 + b) * QG_ROWS] = v[b];
                 }
             }
+            release();
             if (whole || finisher) continue;
             __threadfence();
             named_bar_sync(1, 128);
@@ -610,9 +546,6 @@ __global__ void __launch_bounds__(QG_THREADS, 1) qgemm_kernel(const __grid_const
         }
         if (warp == QG_W_EPI0 && lane == 0) q_stamp(p, 7);                    // epilogue done
     }
-    q_fence_before();
-    __syncthreads();
-    if (warp == 3) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(QG_TMEM_COLS) : "memory");
 }
 
 // ---- load time: native GGUF rows -> QG qtile stream -----------------------------------------------------------------------
@@ -671,9 +604,8 @@ int max_clusters_nb() {
     }();
     return n;
 }
-// Cluster mode pays where tiles are few and deep.  With many tiles per cluster (gate/up: 7 rounds, lm_head: 31) it LOST to
-// stream-K on the measurement (run S: gate/up 28 -> 32 us, lm_head 92 -> 138 us): 132 of 148 SMs hold a cluster, the rounds
-// quantise (7 x 4 qtiles against 24.2), and a 4-qtile segment per tile leaves the accumulator hand-off no slack.  Default: at
+// Cluster mode pays where tiles are few and deep.  With many tiles per cluster (gate/up: 7 rounds, lm_head: 31) the rounds
+// quantise (7 x 4 qtiles against 24.2 under stream-K) and a 4-qtile segment per tile leaves the accumulator hand-off no slack.  Default: at
 // most two rounds (QKV, attn_output, ffn_down of the Llama shapes); GL_QGEMM_CLUSTER_ROUNDS overrides.
 int cluster_max_rounds() {
     static const int r = []() { const char* e = getenv("GL_QGEMM_CLUSTER_ROUNDS"); const int v = e ? atoi(e) : 2; return v < 1 ? 1 : v; }();
@@ -687,8 +619,8 @@ bool cluster_mode_enabled() {
 template <int NB>
 cudaError_t launch_nb(QParams& qp, int grid, int n_sm, cudaStream_t s) {
     // Tile-aligned split-K inside clusters of four.  Under stream-K a tile of QKV / attn_output / ffn_down (32-48 tiles of 16-56
-    // K-blocks on 148 SMs) is shared by 4-6 CTAs that all finish at the same moment, and the partial sums cross L2 on the
-    // critical path (7-10 us per launch, run M); a cluster exchanges them through distributed shared memory.  Stream-K remains
+    // K-blocks on 132 SMs) is shared by 4-6 CTAs that all finish at the same moment, and the partial sums cross L2 on the
+    // critical path; a cluster exchanges them through distributed shared memory.  Stream-K remains
     // for GEMMs with many tiles per cluster (gate/up, lm_head: cluster_max_rounds()), for matrices with fewer than four K-blocks
     // per row and for GL_QGEMM_CLUSTER=0.
     qp.ck_s = 0;

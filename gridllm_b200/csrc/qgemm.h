@@ -41,7 +41,7 @@ struct QGemmWeights {
 // source of rows for the load-time packer: a matrix in NATIVE GGUF row layout on the device
 struct QGemmSource { const uint8_t* w; int type; int rows; };
 
-constexpr int QGEMM_MAX_GRID = 148;
+constexpr int QGEMM_MAX_GRID = 132;       // one CTA per SM of an H100 SXM
 
 // RMSNorm folded into the GEMMs around it (no separate kernel, no launch boundary):
 //   the residual-add GEMM in front of a norm (attn_output, ffn_down) also writes xg[b][n] = fp16(x_new[b][n] * gamma[n] / 16) -- the

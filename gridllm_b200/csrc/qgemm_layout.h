@@ -11,8 +11,8 @@
 //   plane  : inside a qtile the fields of the 128 super-blocks are regrouped into planes of [128 rows][16 B], so that the 32
 //            lanes of a warp (32 consecutive rows) read 512 contiguous bytes per 128-bit load -- no bank conflicts, no 2-byte
 //            aligned 210-byte records
-//   K-step : 64 columns = one tcgen05 A operand [128 rows x 64] fp16 -- kept in TENSOR MEMORY (lane = row, 32 columns of two
-//            fp16 each), written by the unpack warps with tcgen05.st, never staged in shared memory; a qtile is 4 K-steps
+//   K-step : 64 columns = one wgmma A operand [128 rows x 64] fp16 in shared memory (128-byte swizzle), written by the unpack
+//            warps; a qtile is 4 K-steps
 //   chunk  : 8 consecutive columns of one row = four packed half2 words
 //
 // QG layouts (a lossless permutation of the GGUF bits; pack_block() below is the definition):
@@ -230,7 +230,7 @@ QG_FN uint16_t qg_ld16(const uint8_t* p) { uint16_t v; memcpy(&v, p, 2); return 
 // ---- the per-thread program of the kernel's unpack warps -------------------------------------------------------------------
 // Thread (row r, K-step kk) turns columns 64kk..64kk+63 of row r's super-block into 8 chunks of 8 fp16 (four packed half2 words
 // each) and hands them to `store(c, words)`, c = 0..7 in column order.  The kernel collects the 32 words in registers and writes
-// them to TENSOR MEMORY (the A operand of the MMA: lane = row, column = k / 2); the host check writes them to a plain array.
+// them to shared memory (the A operand of the MMA: row r, fp16 columns in order); the host check writes them to a plain array.
 // `raw` is the qtile image (shared memory on the device).
 template <typename StoreChunk>
 QG_FN void qg_dequant_kstep(int type, const uint8_t* raw, int r, int kk, StoreChunk store) {

@@ -1,5 +1,5 @@
 /*
- * gridllm_native.h -- C ABI of libgridllm_native.so, the B200-native inference engine that
+ * gridllm_native.h -- C ABI of libgridllm_native.so, the H100-native inference engine that
  * replaces the GridLLM worker's Ollama HTTP call-out.
  *
  * The reference has no FFI today: the seam is the TypeScript class OllamaService

@@ -165,8 +165,8 @@ extern "C" int hc_detokenize(const char* gguf_path, const int32_t* ids, int n, c
 }
 
 // ---- batched decode GEMM on quantised weights (qgemm_layout.h): pack 128 GGUF super-blocks into a qtile, run the kernel's
-// per-thread dequantisation program for all 256 (row, half) threads into four swizzled operand tiles, un-swizzle with the
-// TMA / tcgen05 128-byte-swizzle rule and hand back the fp16 bit patterns [128 rows][256 columns] ------------------------------
+// per-thread dequantisation program for every (row, K-step) of the qtile and hand back the fp16 bit patterns [128 rows][256 columns]
+// in column order (the kernel stores the same chunks into 128-byte-swizzled shared-memory operand tiles) -------------------------
 #include "../../gridllm_b200/csrc/qgemm_layout.h"
 extern "C" int hc_qg_dequant(int type, const uint8_t* blocks /*[128][block bytes]*/, uint16_t* out /*[128][256]*/, int* qtile_bytes) {
     if (!qg_type_ok(type)) return -1;
@@ -175,11 +175,11 @@ extern "C" int hc_qg_dequant(int type, const uint8_t* blocks /*[128][block bytes
     for (int r = 0; r < QG_ROWS; ++r) qg_pack_block(type, blocks + (size_t)r * bb, qt.data(), r);
     *qtile_bytes = qg_qtile_bytes(type);
     std::vector<int> written((size_t)QG_ROWS * QG_COLS / 8, 0);
-    for (int kk = 0; kk < 4; ++kk)                                           // the kernel's 512 unpack threads: (row, K-step)
+    for (int kk = 0; kk < 4; ++kk)                                           // the kernel's unpack threads: (row, half) run K-steps 2 half, 2 half + 1
         for (int r = 0; r < QG_ROWS; ++r)
             qg_dequant_kstep(type, qt.data(), r, kk, [&](int c, QgU4 v) {
                 // chunk c of K-step kk = columns 64kk + 8c .. +7 of row r: words in column order, two fp16 per word (low half first) --
-                // exactly what tcgen05.st puts into TMEM columns 4c .. 4c+3 of the row's lane
+                // exactly the 16 bytes the kernel stores at chunk position c ^ (r % 8) of row r in K-step kk's operand tile
                 memcpy(out + (size_t)r * QG_COLS + 64 * kk + 8 * c, &v, 16);
                 ++written[((size_t)r * QG_COLS + 64 * kk + 8 * c) / 8];
             });

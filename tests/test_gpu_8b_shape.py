@@ -81,7 +81,7 @@ def test_batched_prefill_at_the_benchmarked_shape(engine_8b, oracle_8b):
     toks = np.random.Generator(np.random.PCG64(31337)).integers(0, 128000, size=16)
     ref = _oracle_run(oracle_8b, toks, 1)[-1]
     engine_8b.kv_reset()
-    lg = engine_8b.prefill(toks)                                       # tcgen05 GEMMs on the resident 16-bit weights
+    lg = engine_8b.prefill(toks)                                       # wgmma GEMMs on the resident 16-bit weights
     scale = float(np.abs(ref).max())
     assert np.isfinite(lg).all() and float(np.abs(lg - ref).max()) <= 1e-2 * scale
     if _margin(ref) > 5e-2:

@@ -180,7 +180,7 @@ def test_batched_prefill_matches_oracle(fixture, n_tok, request):
 @pytest.fixture(scope="module")
 def wide_ffn_gguf(tmp_models):
     """One layer, d = 256, n_ff = 6400: with a 300-token prompt the gate/up GEMM has 3 x 100 output tiles -- more than two
-    per SM, so the persistent tcgen05 kernel reuses both halves of its double-buffered TMEM accumulator and its TMA ring
+    per SM, so the persistent wgmma kernel walks several tiles per CTA, reuses its accumulator staging and its TMA ring
     runs on across tile boundaries."""
     from oracle import gguf_synth as S
     shape = S.LlamaShape("wide-ffn-synth", 1, 256, 4, 2, 6400, 512, 10000.0, 1e-5, 512)
@@ -199,7 +199,7 @@ def test_batched_prefill_many_tiles_per_sm(wide_ffn_gguf, n_tok, monkeypatch):
         ref = orc.step(int(t))
     scale = np.abs(ref).max()
     e = _engine(wide_ffn_gguf, prefill_mode=0)
-    for _ in range(2):                                   # twice: barriers / TMEM are set up per launch
+    for _ in range(2):                                   # twice: barriers are set up per launch
         e.kv_reset()
         lb = e.prefill(toks)
         assert np.isfinite(lb).all()
@@ -239,28 +239,6 @@ def test_fused_prompt_attention_equals_three_launch_path(fixture, n_tok, request
     assert np.abs(d1 - d0).max() <= 2e-3 * np.abs(d0).max()
 
 
-@pytest.mark.parametrize("n_tok", [37, 128, 300, 700])
-def test_tcgen05_prompt_attention_equals_the_mma_sync_kernel(tiny128_gguf, n_tok, monkeypatch):
-    """prefill_attn_tc5.cu (S, P and O in tensor memory, tcgen05.mma with the probabilities as the TMEM A operand,
-    GL_PREFILL_ATTN_TC5=1) against prefill_attn.cu's mma.sync kernel on the same q / k / v bits: both round P to fp16 and sum the
-    rounded values; KV tiles are 128 instead of 64 rows, so the online-softmax rescaling points differ -- 2e-3 * max|logit|.
-    1 .. 6 query tiles: one KV tile (diagonal only), both TMEM score buffers in use, the third tile re-using the first buffer."""
-    from oracle import llama_oracle as O
-    m = O.load_gguf(tiny128_gguf)
-    toks = np.random.Generator(np.random.PCG64(8000 + n_tok)).integers(0, m.n_vocab - 3, size=n_tok)
-    out = {}
-    for mode in ("1", "0"):
-        monkeypatch.setenv("GL_PREFILL_ATTN_TC5", mode)
-        e = _engine(tiny128_gguf, prefill_mode=0, max_ctx=1024)
-        for _ in range(2):                                   # twice: barriers / TMEM are set up per launch
-            e.kv_reset()
-            out[mode] = e.prefill(toks)
-        e.close()
-    scale = np.abs(out["0"]).max()
-    assert np.isfinite(out["1"]).all()
-    assert np.abs(out["1"] - out["0"]).max() <= 2e-3 * scale, (n_tok, np.abs(out["1"] - out["0"]).max(), scale)
-
-
 @pytest.mark.parametrize("fixture", ["tiny_gguf", "tiny128_gguf"])
 @pytest.mark.parametrize("n_tok", [37, 300])
 def test_rope_split_in_the_qkv_epilogue_equals_the_kernel(fixture, n_tok, request, monkeypatch):
@@ -284,26 +262,6 @@ def test_rope_split_in_the_qkv_epilogue_equals_the_kernel(fixture, n_tok, reques
     assert np.isfinite(out["1"][0]).all() and np.isfinite(out["1"][1]).all()
     assert np.abs(out["1"][0] - out["0"][0]).max() <= 2e-3 * scale, (fixture, n_tok, np.abs(out["1"][0] - out["0"][0]).max(), scale)
     assert np.abs(out["1"][1] - out["0"][1]).max() <= 2e-3 * np.abs(out["0"][1]).max()
-
-
-@pytest.mark.parametrize("n_tok", [129, 300, 520])
-def test_cta_pair_gemm_equals_single_cta_gemm(wide_ffn_gguf, n_tok, monkeypatch):
-    """tcgen05.mma.cta_group::2 (256 x 256 tiles on two SMs, GL_TC5_PAIR=2: wherever the shape allows) against the one-CTA kernel: same operands, same K
-    order per output element.  Ragged M: the pair's second CTA owns rows past the prompt in the last tile."""
-    from oracle import llama_oracle as O
-    m = O.load_gguf(wide_ffn_gguf)
-    toks = np.random.Generator(np.random.PCG64(6000 + n_tok)).integers(0, m.n_vocab - 3, size=n_tok)
-    out = {}
-    for mode in ("2", "0"):                               # 2 = pairs whenever the shape allows, 0 = never
-        monkeypatch.setenv("GL_TC5_PAIR", mode)
-        e = _engine(wide_ffn_gguf, prefill_mode=0, max_ctx=1024)
-        for _ in range(2):
-            e.kv_reset()
-            out[mode] = e.prefill(toks)
-        e.close()
-    scale = np.abs(out["0"]).max()
-    assert np.isfinite(out["2"]).all()
-    assert np.abs(out["2"] - out["0"]).max() <= 1e-5 * scale, (n_tok, np.abs(out["2"] - out["0"]).max(), scale)
 
 
 def test_generate_with_batched_prefill(tiny128_gguf):

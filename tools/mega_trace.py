@@ -21,7 +21,7 @@ def main():
     ctx = int(sys.argv[1]) if len(sys.argv) > 1 else 576
     ms, _ = e.time_decode(ctx, 8)
     lib = N.load_library()
-    cap = 148 * 200 * 4
+    cap = 132 * 200 * 4
     buf = np.zeros(cap, dtype=np.uint64)
     nc, nph = C.c_int32(), C.c_int32()
     rc = lib.gl_debug_mega_trace(e._h, buf.ctypes.data_as(C.c_void_p), cap, C.byref(nc), C.byref(nph))

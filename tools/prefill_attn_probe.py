@@ -1,6 +1,6 @@
 """Prompt-pass probe on the GPU box: the Llama-3-8B-shaped model's batched prefill under a list of switch settings
 (PROBE_VARIANTS="GL_PREFILL_FLASH=1;GL_PREFILL_FLASH=0" by default: the fused attention kernel of prefill_attn.cu against the
-three-launch path; "GL_TC5_PAIR=1;GL_TC5_PAIR=0": CTA-pair GEMM against the one-CTA kernel), at the prompt lengths given on the
+three-launch path), at the prompt lengths given on the
 command line: device time of the prompt pass and agreement of the first generated token's logits with the first variant's."""
 import json
 import os

@@ -1,5 +1,5 @@
 """Prefill probe on the GPU box: 512-token prompt of the Llama-3-8B-shaped model through the batched prefill with the
-tcgen05 GEMM and with the mma.sync GEMM; time and agreement of the first generated token's logits."""
+wgmma GEMM and with the mma.sync GEMM; time and agreement of the first generated token's logits."""
 import json
 import os
 import sys

@@ -1,8 +1,8 @@
-"""Device timeline of the quantised GEMMs inside one REPLAYED batched step (run on the GPU box with GL_QGEMM_TRACE=1).
+"""Device timeline of the quantised GEMMs inside one REPLAYED batched step (run on an H100 with GL_QGEMM_TRACE=1).
 
 The kernel stamps %globaltimer per CTA at: 0 entry, 1 prologue done, 2 first weight copy issued, 3 first qtile landed,
-4/5 unpack groups done, 6 last accumulator complete, 7 epilogue done, 8 upstream kernel complete (griddepcontrol.wait
-returned), 9 last MMA issued.  A captured graph keeps the trace slot of its capture, so after the replays the buffer holds
+4 unpack warps done (5 is not written), 6 last accumulator complete, 7 epilogue done, 8 upstream kernel complete
+(griddepcontrol.wait returned), 9 last MMA complete.  A captured graph keeps the trace slot of its capture, so after the replays the buffer holds
 the stamps of the LAST replay of every launch.  usage: qgemm_trace.py <batch> <ctx>"""
 import ctypes
 import os
@@ -14,8 +14,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 os.environ["GL_QGEMM_TRACE"] = "1"
 
-SLOTS, GRID = 10, 148
-NAMES = ["entry", "prologue", "tma0", "qtile0", "unpack_g0", "unpack_g1", "acc_last", "epi_done", "upstream_done", "mma_last"]
+SLOTS, GRID = 10, 132
+NAMES = ["entry", "prologue", "tma0", "qtile0", "unpack_done", "unused", "acc_last", "epi_done", "upstream_done", "mma_last"]
 
 
 def main():
@@ -54,8 +54,8 @@ def main():
         end = rel[:, 7].max()
         nxt = (t[k + 1][:, 0][t[k + 1][:, 0] > 0].min() - base) / 1e3 if k + 1 < len(t) else float("nan")
         rows.append(dict(ctas=int(m.sum()), entry_max=rel[:, 0].max(), prologue=np.median(rel[:, 1]), tma0=np.median(rel[:, 2]),
-                         upstream=np.median(rel[:, 8]), qtile0=np.median(rel[:, 3]), unpack_med=np.median(np.maximum(rel[:, 4], rel[:, 5])),
-                         unpack_max=np.maximum(rel[:, 4], rel[:, 5]).max(), mma_last=np.median(rel[:, 9]), acc_med=np.median(rel[:, 6]),
+                         upstream=np.median(rel[:, 8]), qtile0=np.median(rel[:, 3]), unpack_med=np.median(rel[:, 4]),
+                         unpack_max=rel[:, 4].max(), mma_last=np.median(rel[:, 9]), acc_med=np.median(rel[:, 6]),
                          acc_max=rel[:, 6].max(), epi_med=np.median(rel[:, 7]), end=end, next_entry=nxt))
     keys = list(rows[0].keys())
     print("launch  " + " ".join("%11s" % k for k in keys))
