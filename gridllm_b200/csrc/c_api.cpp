@@ -2,6 +2,8 @@
 // call site each entry point stands in for.
 #include <cuda_runtime.h>
 
+#include <cmath>
+#include <cstddef>
 #include <cstring>
 #include <new>
 #include <stdexcept>
@@ -25,6 +27,25 @@ int ret(const Status& s) {
 int bad(const char* m) {
     gl::set_last_error(m);
     return GL_ERR_INVALID;
+}
+
+// The penalty fields took the place of six reserved words: the struct's size and the offsets of the older fields are what
+// hosts built against ABI version 2 lay out (a caller that zeroes `reserved` gets no penalty and no min_p).
+static_assert(sizeof(gl_sample_opts) == 72, "gl_sample_opts size is part of the ABI");
+static_assert(offsetof(gl_sample_opts, seed) == 16 && offsetof(gl_sample_opts, stop_ids) == 32 &&
+                  offsetof(gl_sample_opts, want_logits) == 40, "gl_sample_opts offsets are part of the ABI");
+static_assert(offsetof(gl_sample_opts, repeat_penalty) == 44 && offsetof(gl_sample_opts, min_p) == 60 &&
+                  offsetof(gl_sample_opts, reserved) == 64, "penalty fields sit where reserved[0..5] was");
+
+// the penalty / min_p fields of a request (include/gridllm_native.h); nullptr when valid
+const char* check_penalties(const gl_sample_opts& so) {
+    if (!std::isfinite(so.repeat_penalty) || !std::isfinite(so.presence_penalty) || !std::isfinite(so.frequency_penalty) ||
+        !std::isfinite(so.min_p))
+        return "repeat_penalty, presence_penalty, frequency_penalty and min_p must be finite";
+    if (so.repeat_penalty < 0.f) return "repeat_penalty must be >= 0";
+    if (so.repeat_last_n < -1) return "repeat_last_n must be >= -1";
+    if (so.min_p < 0.f || so.min_p > 1.f) return "min_p must lie in [0, 1]";
+    return nullptr;
 }
 }  // namespace
 
@@ -117,6 +138,7 @@ int gl_generate(gl_engine* e, const int32_t* prompt, int32_t n_prompt, const gl_
     gl_sample_opts so{};
     if (opts) so = *opts;
     else { so.num_predict = 128; so.top_p = 1.f; }
+    if (const char* m = check_penalties(so)) return bad(m);
     return ret(e->impl->generate(prompt, n_prompt, so, cb, user, out_ids, out_logprobs, stats));
 }
 
@@ -131,6 +153,7 @@ int gl_seq_open(gl_engine* e, const int32_t* prompt, int32_t n_prompt, const gl_
     gl_sample_opts so{};
     if (opts) so = *opts;
     else { so.num_predict = 128; so.top_p = 1.f; }
+    if (const char* m = check_penalties(so)) return bad(m);
     int s = -1;
     const int rc = ret(e->impl->seq_open(prompt, n_prompt, so, &s));
     if (rc == GL_OK) *slot = s;
@@ -140,6 +163,8 @@ int gl_seq_open(gl_engine* e, const int32_t* prompt, int32_t n_prompt, const gl_
 int gl_seq_open_many(gl_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seq, const gl_sample_opts* opts, int32_t* slots,
                      int32_t* n_opened) {
     if (!e || !ids || !offsets || !opts || !slots || !n_opened) return bad("gl_seq_open_many: null argument");
+    for (int32_t i = 0; i < n_seq; ++i)
+        if (const char* m = check_penalties(opts[i])) return bad(m);
     int k = 0;
     const int rc = ret(e->impl->seq_open_many(ids, offsets, n_seq, opts, slots, &k));
     *n_opened = k;
@@ -213,10 +238,17 @@ int gl_last_logits(gl_engine* e, int32_t step, float* out, int32_t n_vocab) {
 int gl_sample_logits(gl_engine* e, const float* logits, int32_t n_vocab, const gl_sample_opts* opts, int32_t out_index, int32_t* id,
                      float* logprob) {
     if (!e || !logits || !opts) return bad("gl_sample_logits: null argument");
+    if (const char* m = check_penalties(*opts)) return bad(m);
     int tid = 0;
     const int rc = ret(e->impl->sample_logits(logits, n_vocab, *opts, out_index, &tid, logprob));
     if (rc == GL_OK && id) *id = tid;
     return rc;
+}
+
+int gl_penalize_logits(gl_engine* e, float* logits, int32_t n_vocab, const gl_sample_opts* opts, const int32_t* history, int32_t n_history) {
+    if (!e || !logits || !opts) return bad("gl_penalize_logits: null argument");
+    if (const char* m = check_penalties(*opts)) return bad(m);
+    return ret(e->impl->penalize_logits(logits, n_vocab, *opts, history, n_history));
 }
 
 int gl_gemv(gl_engine* e, int ggml_type, const void* w_host, int32_t rows, int32_t cols, const float* x, float* y, int32_t iters,

@@ -24,6 +24,11 @@ struct StepState {
     int top_k;          // <= 0 or > SAMPLE_MAX_K: the SAMPLE_MAX_K best logits
     float top_p;        // 1 = off
     unsigned seed_lo, seed_hi;
+    float min_p;        // 0 = off (temperature > 0 only)
+    // repetition penalties (penalty.cu); pen_last_n = 0: none (the host also sets it to 0 when every penalty is a no-op)
+    int pen_last_n;     // window: > 0 the last N history ids, -1 the whole history
+    float repeat_penalty;     // 1 = off
+    float presence_penalty, frequency_penalty;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }

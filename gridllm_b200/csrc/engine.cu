@@ -79,10 +79,12 @@ Engine::~Engine() {
     if (stream_) cudaStreamSynchronize(stream_);
     if (g_nohead_) cudaGraphExecDestroy(g_nohead_);
     for (auto& v : g_head_var_)
+        for (auto& k : v)
+            for (auto& g : k)
+                if (g) cudaGraphExecDestroy(g);
+    for (auto& v : g_batch_)
         for (auto& g : v)
             if (g) cudaGraphExecDestroy(g);
-    for (auto& g : g_batch_)
-        if (g) cudaGraphExecDestroy(g);
     for (auto& ev : ev_) if (ev) cudaEventDestroy(ev);
     for (void* p : allocs_) cudaFree(p);
     for (void* p : pf_allocs_) cudaFree(p);
@@ -302,6 +304,7 @@ Status Engine::load(const std::string& path, int device, const gl_engine_opts* o
     CU(dalloc((void**)&counters_, (size_t)n_kv_ * 4));
     CU(dalloc((void**)&sample_scratch_, (size_t)SAMPLE_SCRATCH_FLOATS * 4));
     CU(dalloc((void**)&topk_scratch_, TOPK_SCRATCH_BYTES));
+    CU(dalloc((void**)&pen_counts_, (size_t)n_vocab_ * 4));
     n_pages_ = n_ctx_ / KV_PAGE_TOKENS;
     // the page pool is shared by every open sequence (gl_generate's one sequence and the gl_seq_open slots)
     max_batch_ = std::max(0, std::min(MAX_BATCH, env_int("GL_MAX_BATCH", opts ? opts->max_batch : 0)));
@@ -425,7 +428,7 @@ Status Engine::ensure_pages(int n_tokens) {
     return {};
 }
 
-StepState Engine::make_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so, int* sampler) const {
+StepState Engine::make_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so, int* sampler, int* penalised) const {
     StepState h{};
     h.pos = pos; h.token = token; h.n_prompt = n_prompt; h.out_idx = out_idx; h.done = 0;
     h.ignore_eos = so ? so->ignore_eos : 1;
@@ -443,11 +446,21 @@ StepState Engine::make_state(int pos, int token, int n_prompt, int out_idx, cons
     h.top_p = (so && so->top_p > 0.f) ? so->top_p : 1.f;
     h.seed_lo = so ? (unsigned)(so->seed & 0xffffffffull) : 0u;
     h.seed_hi = so ? (unsigned)(so->seed >> 32) : 0u;
+    h.min_p = (so && so->min_p > 0.f) ? so->min_p : 0.f;
+    // repetition penalties (penalty.cu): repeat_penalty is active when > 0 and != 1; a window of 0, or nothing active, is no
+    // penalty at all, and such a request replays exactly the graphs of a request without the fields
+    const bool rp_on = so && so->repeat_penalty > 0.f && so->repeat_penalty != 1.f;
+    const bool pen = so && so->repeat_last_n != 0 && (rp_on || so->presence_penalty != 0.f || so->frequency_penalty != 0.f);
+    h.pen_last_n = pen ? so->repeat_last_n : 0;
+    h.repeat_penalty = rp_on ? so->repeat_penalty : 1.f;
+    h.presence_penalty = pen ? so->presence_penalty : 0.f;
+    h.frequency_penalty = pen ? so->frequency_penalty : 0.f;
+    if (penalised) *penalised = pen ? 1 : 0;
     return h;
 }
 
 Status Engine::set_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so) {
-    const StepState h = make_state(pos, token, n_prompt, out_idx, so, &sampler_);
+    const StepState h = make_state(pos, token, n_prompt, out_idx, so, &sampler_, &penalised_);
     if (bar_counter_) CU(cudaMemsetAsync(bar_counter_, 0, 4, stream_));
     CU(cudaMemcpyAsync(st_, &h, sizeof(h), cudaMemcpyHostToDevice, stream_));
     CU(cudaStreamSynchronize(stream_));     // h is on the stack
@@ -603,6 +616,11 @@ Status Engine::enqueue_head(cudaStream_t s, bool keep_logits, int* n_launch) {
         CU(rmsnorm_launch(x_, output_norm_, n_embd_, eps_, xn_, s)); ++*n_launch;
         ST(plain_gemv(s, output_, xn_, logits_, n_launch));
     }
+    if (penalised_) {          // repetition penalties on the logits before the draw (penalty.cu); plain stream order after the lm_head
+        PenaltyParams pp{logits_, n_vocab_, st_, nullptr, prompt_ids_, 0, out_ids_, 0, pen_counts_};
+        CU(penalty_launch(pp, 1, false, s));
+        ++*n_launch;
+    }
     SampleParams sp{logits_, n_vocab_, st_, out_ids_, out_lp_, keep_logits ? logits_keep_ : nullptr, keep_logits ? keep_cap_ : max_out_, sample_scratch_, topk_scratch_};
     if (sampler_ != 0) CU(sample_topk_launch(sp, sampler_ == 1, pdl && fused_ && sampler_pdl_, s));      // temperature > 0: seeded top-k / top-p draw (sampler.cu)
     else CU(sample_greedy_launch(sp, pdl && fused_ && greedy_pdl_, s));
@@ -623,7 +641,7 @@ Status Engine::build_graphs() {
         e = cudaGraphInstantiate(&ge, g, 0);
         cudaGraphDestroy(g);
         if (e != cudaSuccess) return fail(GL_ERR_CUDA, std::string("graph instantiate: ") + cudaGetErrorString(e));
-        if (which == 0) { g_nohead_ = ge; launches_nohead_ = n; } else { g_head_var_[0][0] = ge; launches_head_ = n; }
+        if (which == 0) { g_nohead_ = ge; launches_nohead_ = n; } else { g_head_var_[0][0][0] = ge; launches_head_ = n; }
     }
     return {};
 }
@@ -635,8 +653,9 @@ Status Engine::run_steps(int n_nohead, int n_head, bool keep_logits) {
         if (n_head > 0) ST(launch_mega(n_head, true, keep_logits));
         return {};
     }
-    // the step with a head exists in six captured variants (sampler x plain / logits kept); all but the first lazily
-    cudaGraphExec_t* head = &g_head_var_[sampler_][keep_logits ? 1 : 0];
+    // the step with a head exists in twelve captured variants (sampler x plain / logits kept x without / with the penalty
+    // kernel); all but the first lazily
+    cudaGraphExec_t* head = &g_head_var_[sampler_][keep_logits ? 1 : 0][penalised_ ? 1 : 0];
     if (use_graph_ && n_head > 0 && !*head) {
         cudaGraph_t g = nullptr;
         CU(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
@@ -780,6 +799,11 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
     const int n_pred = so.num_predict > 0 ? so.num_predict : 128;     // OllamaService.ts:105
     if (!(so.temperature >= 0.f) || !std::isfinite(so.temperature)) return fail(GL_ERR_INVALID, "temperature must be a finite number >= 0");
     if (so.temperature > 0.f && use_mega_) return fail(GL_ERR_UNSUPPORTED, "the persistent decode kernel (GL_MEGA=1) samples greedily only");
+    if (use_mega_) {
+        int pen = 0;
+        make_state(0, 0, n_prompt, 0, &so, nullptr, &pen);
+        if (pen) return fail(GL_ERR_UNSUPPORTED, "the persistent decode kernel (GL_MEGA=1) has no repetition penalties");
+    }
     for (int i = 0; i < n_prompt; ++i)
         if (prompt[i] < 0 || prompt[i] >= n_vocab_) return fail(GL_ERR_INVALID, "prompt token id out of range");
     ST(kv_reset());
@@ -792,7 +816,8 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
             logits_keep_ = p;
             keep_cap_ = n_pred;
             for (auto& v : g_head_var_)
-                if (v[1]) { cudaGraphExecDestroy(v[1]); v[1] = nullptr; }      // captured with the old logits buffer
+                for (auto& g : v[1])
+                    if (g) { cudaGraphExecDestroy(g); g = nullptr; }      // captured with the old logits buffer
         }
     }
     CU(cudaMemcpyAsync(prompt_ids_, prompt, (size_t)n_prompt * 4, cudaMemcpyHostToDevice, stream_));
@@ -865,7 +890,7 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
         stats->load_duration_ns = load_ns_;
         stats->done_reason = done_reason;
         stats->kernel_launches = use_mega_ ? prefill_launches + (mega_launches_ - mega0) + (batched ? 2 : 0)
-                                           : prefill_launches + std::max(produced, 1) * launches_head_;
+                                           : prefill_launches + std::max(produced, 1) * head_launches();
     }
     return cancelled ? fail(GL_ERR_CANCELLED, "cancelled by token callback") : Status{};
 }
@@ -899,6 +924,37 @@ Status Engine::sample_logits(const float* logits, int n_vocab, const gl_sample_o
     if (id) *id = tid;
     if (logprob) *logprob = lp;
     return {};
+}
+
+// The penalty kernel alone on caller-supplied logits with a caller-supplied history (parity tests against tests/penalty_oracle.py):
+// the history is the "prompt" of a sequence that has drawn nothing yet.  Rewinds the sequence.
+Status Engine::penalize_logits(float* logits, int n_vocab, const gl_sample_opts& so, const int32_t* history, int n_history) {
+    CU(cudaSetDevice(device_));
+    if (!logits || n_vocab != n_vocab_) return fail(GL_ERR_INVALID, "logits must hold n_vocab values");
+    if (n_history < 0 || (n_history > 0 && !history)) return fail(GL_ERR_INVALID, "bad history");
+    for (int i = 0; i < n_history; ++i)
+        if (history[i] < 0 || history[i] >= n_vocab_) return fail(GL_ERR_INVALID, "history token id out of range");
+    ST(kv_reset());
+    gl_sample_opts o = so;
+    o.ignore_eos = 1;
+    ST(set_state(0, 0, n_history, 0, &o));
+    int* hist = nullptr;
+    if (n_history > 0) CU(cudaMalloc((void**)&hist, (size_t)n_history * 4));
+    Status rs;
+    do {
+        cudaError_t ce = hist ? cudaMemcpyAsync(hist, history, (size_t)n_history * 4, cudaMemcpyHostToDevice, stream_) : cudaSuccess;
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(logits_, logits, (size_t)n_vocab_ * 4, cudaMemcpyHostToDevice, stream_);
+        if (ce == cudaSuccess && penalised_ && hist) {
+            PenaltyParams pp{logits_, n_vocab_, st_, nullptr, hist, 0, out_ids_, 0, pen_counts_};
+            ce = penalty_launch(pp, 1, false, stream_);
+        }
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(logits, logits_, (size_t)n_vocab_ * 4, cudaMemcpyDeviceToHost, stream_);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(stream_);
+        if (ce != cudaSuccess) rs = fail(GL_ERR_CUDA, std::string("penalize_logits: ") + cudaGetErrorString(ce));
+    } while (false);
+    if (hist) cudaFree(hist);
+    ST(rs);
+    return kv_reset();
 }
 
 Status Engine::decode_step(int token, float* logits, int* argmax, float* logprob) {

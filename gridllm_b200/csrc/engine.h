@@ -70,6 +70,7 @@ public:
     }
     Status time_batch_step(int batch, int ctx_len, int iters, float* ms, int* launches, uint64_t* wbytes);
     Status sample_logits(const float* logits, int n_vocab, const gl_sample_opts& so, int out_index, int* id, float* logprob);
+    Status penalize_logits(float* logits, int n_vocab, const gl_sample_opts& so, const int32_t* history, int n_history);
     Status gemv_host(int type, const void* w_host, int rows, int cols, const float* x, float* y, int iters, float* ms);
     Status gemv_tensor(const std::string& name, const float* x, float* y, int iters, int flush, float* ms, uint64_t* wbytes);
     Status rmsnorm(const float* x, const float* w, int n, float eps, float* y);
@@ -93,7 +94,8 @@ private:
     Status plain_gemv(cudaStream_t s, const DevMatrix& m, const float* x, float* y, int* n_launch);
     Status build_graphs();
     Status set_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so);
-    StepState make_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so, int* sampler) const;
+    // *penalised (optional): 1 when the request's repetition penalties are not a no-op (penalty.cu must run before its draws)
+    StepState make_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so, int* sampler, int* penalised = nullptr) const;
     Status run_steps(int n_nohead, int n_head, bool keep_logits);
     Status enqueue_head(cudaStream_t s, bool keep_logits, int* n_launch);
     Status build_prefill_weights();
@@ -173,6 +175,7 @@ private:
     float *part_o_ = nullptr, *part_ml_ = nullptr;
     unsigned* counters_ = nullptr;
     float* sample_scratch_ = nullptr;
+    int* pen_counts_ = nullptr;                      // [n_vocab] penalty.cu count scratch of the single-sequence path (zero between launches)
     unsigned long long* topk_scratch_ = nullptr;
     __half *kcache_ = nullptr, *vcache_ = nullptr;    // [layer][page][kv][16][hd]
     size_t kv_layer_elems_ = 0;
@@ -196,7 +199,7 @@ private:
     struct SeqSlot {
         bool open = false, done = false, first_pending = false;
         std::vector<int> pages;
-        int n_prompt = 0, n_pred = 0, produced = 0, sampler = 0;
+        int n_prompt = 0, n_pred = 0, produced = 0, sampler = 0, penalised = 0;
         int32_t last_token = 0;
         float first_lp = 0.f;
         int last_row = -1;                            // row of the last batched step this sequence took part in
@@ -215,6 +218,8 @@ private:
     StepState* bst_ = nullptr;                        // [MAX_BATCH]
     int* btables_ = nullptr;                          // [MAX_BATCH][n_pages_]
     int *bids_ = nullptr, *bout_ids_ = nullptr;
+    int* bprompt_ = nullptr;                          // [max_batch][n_ctx] each slot's prompt ids (the head of its penalty history)
+    int* bpen_counts_ = nullptr;                      // [max_batch][n_vocab] penalty.cu count scratch per slot (zero between launches)
     static constexpr int BSSQ_PARTS = 512;       // 32-row slices of the residual stream the folded RMSNorm can sum (n_embd <= 16 384)
     float* bssq_[2] = {nullptr, nullptr};
     float *bx_ = nullptr, *bqkv_ = nullptr, *bq_ = nullptr, *blogits_ = nullptr, *bfirst_logits_ = nullptr, *bout_lp_ = nullptr, *bpart_o_ = nullptr, *bpart_ml_ = nullptr, *bsample_scratch_ = nullptr;
@@ -231,24 +236,29 @@ private:
     std::string qg_why_not_;                          // why the quantised path is unavailable for this model (message for batch_weights = 2)
     Status build_qgemm_weights();
     Status pack_qgemm(const std::vector<const GGUFTensor*>& src, int mode, QGemmWeights& out, uint8_t*& tmp, size_t& tmp_cap);
-    cudaGraphExec_t g_batch_[N_BUCKETS] = {};
-    int batch_launches_ = 0;                          // kernels of one batched step
+    cudaGraphExec_t g_batch_[N_BUCKETS][2] = {};      // [bucket][1: with the penalty kernel, for steps in which some row has penalties]
+    int batch_launches_ = 0;                          // kernels of one batched step (without the penalty kernel)
     uint64_t bc_[8] = {};                             // gl_batch_counters
     Status ensure_batch_state();
     Status seq_open_single(const int32_t* prompt, int n_prompt, const gl_sample_opts& so, int* slot);
-    Status enqueue_batch_step(cudaStream_t s, int bucket, int* n_launch);
-    Status run_batch_graph(int bucket);
+    Status enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, int* n_launch);
+    Status run_batch_graph(int bucket, bool penalised);
+    cudaError_t batch_penalty_launch(int bucket, cudaStream_t s);
+    Status ensure_batch_penalty();                    // bprompt_ / bpen_counts_, allocated when the first penalised sequence opens
+    Status keep_prompt(int slot, const int32_t* prompt, int n_prompt);     // a penalised slot's prompt -> bprompt_
     static int bucket_of(int rows) { int b = 8; while (b < rows) b <<= 1; return b; }
     static int bucket_index(int bucket) { int i = 0; while ((8 << i) < bucket) ++i; return i; }
 
     cudaGraphExec_t g_nohead_ = nullptr;
-    cudaGraphExec_t g_head_var_[3][2] = {};   // [sampler of the running request][logits kept]
+    cudaGraphExec_t g_head_var_[3][2][2] = {};   // [sampler of the running request][logits kept][repetition penalties]
+    int penalised_ = 0;                        // the running request has penalties: penalty.cu runs between the lm_head and the sampler
     // The top-k samplers are launched WITHOUT programmatic dependent launch: their CTAs (33 KB of shared memory each) resident
     // beside the lm_head CTAs cost the step 60 us (run 67: 1.537 -> 1.478 ms/token at top_k 40); the greedy sampler keeps it.
     bool sampler_pdl_ = false;
     bool greedy_pdl_ = false;                 // the greedy sampler likewise (64 small CTAs: 3 us per token, run 68)
     int sampler_ = 0;                          // 0 greedy (argmax), 1 / 2: the two kernels of sampler.cu (temperature > 0)
-    int launches_nohead_ = 0, launches_head_ = 0;
+    int launches_nohead_ = 0, launches_head_ = 0;    // launches_head_: the step with a head WITHOUT the penalty kernel
+    int head_launches() const { return launches_head_ + (penalised_ && !use_mega_ ? 1 : 0); }     // ... of the variant that runs
     cudaEvent_t ev_[4] = {nullptr, nullptr, nullptr, nullptr};
     int64_t load_ns_ = 0;
     uint64_t weight_bytes_ = 0, decode_bytes_ = 0, n_params_ = 0;

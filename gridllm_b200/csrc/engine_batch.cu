@@ -180,11 +180,40 @@ Status Engine::ensure_batch_state() {
     // launch configuration is validated -- and every lazily initialised driver entry point touched -- OUTSIDE stream capture,
     // where an error has a name
     int nl = 0;
-    ST(enqueue_batch_step(stream_, 8, &nl));
+    ST(enqueue_batch_step(stream_, 8, false, &nl));
     CU(cudaStreamSynchronize(stream_));
     batch_launches_ = nl;
     batch_ready_ = true;
     return {};
+}
+
+Status Engine::ensure_batch_penalty() {
+    if (bpen_counts_) return {};
+    int* pr = nullptr;
+    int* cnt = nullptr;
+    CU(cudaMalloc((void**)&pr, (size_t)max_batch_ * n_ctx_ * 4));
+    allocs_.push_back(pr);
+    CU(cudaMalloc((void**)&cnt, (size_t)max_batch_ * n_vocab_ * 4));
+    allocs_.push_back(cnt);
+    CU(cudaMemsetAsync(cnt, 0, (size_t)max_batch_ * n_vocab_ * 4, stream_));
+    bprompt_ = pr;
+    bpen_counts_ = cnt;
+    // one un-captured launch with the current row map (no row, or rows without penalties: every CTA leaves at once) validates the
+    // configuration outside stream capture
+    CU(batch_penalty_launch(8, stream_));
+    return {};
+}
+
+Status Engine::keep_prompt(int slot, const int32_t* prompt, int n_prompt) {
+    ST(ensure_batch_penalty());
+    CU(cudaMemcpyAsync(bprompt_ + (size_t)slot * n_ctx_, prompt, (size_t)n_prompt * 4, cudaMemcpyHostToDevice, stream_));
+    return {};
+}
+
+// the penalty kernel over the rows of a batched step (row r: logits row r, the state / history of slot row_slot[r])
+cudaError_t Engine::batch_penalty_launch(int bucket, cudaStream_t s) {
+    PenaltyParams pp{blogits_, n_vocab_, bst_, bctl_, bprompt_, n_ctx_, bout_ids_, max_out_, bpen_counts_};
+    return penalty_launch(pp, bucket, false, s);
 }
 
 // Prefill a prompt into a free slot's own pages and draw its first token.  The single-sequence code runs unchanged on the
@@ -225,6 +254,16 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
     for (int i = 0; i < need; ++i) { S.pages.push_back(free_pages_.back()); free_pages_.pop_back(); }
     int* table = btables_ + (size_t)slot * n_pages_;
     CU(cudaMemcpyAsync(table, S.pages.data(), S.pages.size() * 4, cudaMemcpyHostToDevice, stream_));
+    int penalised = 0;
+    make_state(0, 0, n_prompt, 0, &so, nullptr, &penalised);
+    if (penalised) {                                 // the head of the history the batched steps penalise with
+        Status ks = keep_prompt(slot, prompt, n_prompt);
+        if (!ks.ok()) {
+            for (int p : S.pages) free_pages_.push_back(p);
+            S = SeqSlot{};
+            return ks;
+        }
+    }
 
     struct Saved { int* pt; StepState* st; int* oi; float* ol; int hp; } sv{page_table_, st_, out_ids_, out_lp_, host_pos_};
     page_table_ = table; st_ = bst_ + slot; out_ids_ = bout_ids_ + (size_t)slot * max_out_; out_lp_ = bout_lp_ + (size_t)slot * max_out_; host_pos_ = 0;
@@ -268,7 +307,7 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
         return rs;
     }
     S.open = true;
-    S.n_prompt = n_prompt; S.n_pred = n_pred; S.produced = 0; S.sampler = sampler; S.first_pending = true;
+    S.n_prompt = n_prompt; S.n_pred = n_pred; S.produced = 0; S.sampler = sampler; S.penalised = penalised; S.first_pending = true;
     S.t_open_ns = t_open; S.launches = prefill_launches; S.stopped = S.done;
     bc_[3] += (uint64_t)S.prefill_ns; bc_[4] += (uint64_t)n_prompt; bc_[5] += 1; bc_[6] += (uint64_t)prefill_launches;
     *slot_out = slot;
@@ -377,17 +416,29 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             std::vector<StepState> hst(P);
             BatchCtl hc{};
             hc.n_rows = P;
+            bool any_pen = false;
             for (int i = 0; i < P && ce == cudaSuccess; ++i) {
                 const int w = which[i], n = lens[i];
-                int sampler = 0;
-                hst[i] = make_state(n - 1, ids[offs[w] + n - 1], n, 0, &opts[w], &sampler);
+                int sampler = 0, pen = 0;
+                hst[i] = make_state(n - 1, ids[offs[w] + n - 1], n, 0, &opts[w], &sampler, &pen);
                 slots_[pslots[i]].sampler = sampler;
+                slots_[pslots[i]].penalised = pen;
+                if (pen) {                                   // the head of the history the penalty kernel reads
+                    Status ks = keep_prompt(pslots[i], ids + offs[w], n);
+                    if (!ks.ok()) { rs = ks; break; }
+                    any_pen = true;
+                }
                 hc.row_slot[i] = pslots[i];
                 ce = cudaMemcpyAsync(bst_ + pslots[i], &hst[i], sizeof(StepState), cudaMemcpyHostToDevice, stream_);
             }
+            if (!rs.ok()) break;
             if (ce == cudaSuccess) ce = cudaMemcpyAsync(bctl_, &hc, sizeof(hc), cudaMemcpyHostToDevice, stream_);
             last_rows_.clear();
             const int bucket = bucket_of(P);
+            if (ce == cudaSuccess && any_pen) {              // penalties before every first-token draw of the pack
+                ce = batch_penalty_launch(bucket, stream_);
+                ++launches;
+            }
             if (ce == cudaSuccess) ce = batch_sample_greedy_launch(blogits_, n_vocab_, bucket, bctl_, bst_, bout_ids_, bout_lp_, max_out_, bsample_scratch_, stream_);
             for (int i = 0; i < P && ce == cudaSuccess; ++i) {
                 const int slot = pslots[i];
@@ -479,7 +530,7 @@ Status Engine::seq_logits(int slot, float* out, int n_vocab) {
 }
 
 // every launch of one batched step, for `bucket` rows; all pointers are fixed, the composition is read from bctl_ / bst_
-Status Engine::enqueue_batch_step(cudaStream_t s, int bucket, int* n_launch) {
+Status Engine::enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, int* n_launch) {
     const int qd = n_head_ * hd_, kvd = n_kv_ * hd_, ldq = qd + 2 * kvd;
     const float scale = 1.0f / std::sqrt((float)hd_);
     int nl = 0;
@@ -560,33 +611,39 @@ Status Engine::enqueue_batch_step(cudaStream_t s, int bucket, int* n_launch) {
         const QGemmNorm nm = consume(bssq_[1]);
         CU(linear(bxn16_, head16_, blogits_, n_vocab_, n_embd_, n_vocab_, GEMM_EPI_F32, use_q ? &qhead_ : nullptr, fold ? &nm : nullptr));
     }
+    // repetition penalties of the rows that have them (penalty.cu), before every sampler of the step: only in the variant used
+    // for steps in which some row has penalties
+    if (penalised) { CU(batch_penalty_launch(bucket, s)); ++nl; }
     CU(batch_sample_greedy_launch(blogits_, n_vocab_, bucket, bctl_, bst_, bout_ids_, bout_lp_, max_out_, bsample_scratch_, s)); ++nl;
     if (n_launch) *n_launch = nl;
     return {};
 }
 
-Status Engine::run_batch_graph(int bucket) {
+// penalised: the variant with the penalty kernel (a second captured step per bucket); batch_launches_ counts the plain one
+Status Engine::run_batch_graph(int bucket, bool penalised) {
     const int bi = bucket_index(bucket);
+    if (penalised && !bpen_counts_) return failb(GL_ERR_INVALID, "batched step: no penalty state");
     if (!use_graph_) {
         int nl = 0;
-        ST(enqueue_batch_step(stream_, bucket, &nl));
-        batch_launches_ = nl;
+        ST(enqueue_batch_step(stream_, bucket, penalised, &nl));
+        batch_launches_ = nl - (penalised ? 1 : 0);
         return {};
     }
-    if (!g_batch_[bi]) {
+    cudaGraphExec_t& ge = g_batch_[bi][penalised ? 1 : 0];
+    if (!ge) {
         cudaGraph_t g = nullptr;
         int nl = 0;
         CU(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
-        Status st = enqueue_batch_step(stream_, bucket, &nl);
+        Status st = enqueue_batch_step(stream_, bucket, penalised, &nl);
         cudaError_t e = cudaStreamEndCapture(stream_, &g);
         if (!st.ok()) { if (g) cudaGraphDestroy(g); return st; }
         if (e != cudaSuccess) return failb(GL_ERR_CUDA, std::string("batched step: graph capture: ") + cudaGetErrorString(e));
-        e = cudaGraphInstantiate(&g_batch_[bi], g, 0);
+        e = cudaGraphInstantiate(&ge, g, 0);
         cudaGraphDestroy(g);
         if (e != cudaSuccess) return failb(GL_ERR_CUDA, std::string("batched step: graph instantiate: ") + cudaGetErrorString(e));
-        batch_launches_ = nl;
+        batch_launches_ = nl - (penalised ? 1 : 0);
     }
-    CU(cudaGraphLaunch(g_batch_[bi], stream_));
+    CU(cudaGraphLaunch(ge, stream_));
     return {};
 }
 
@@ -637,8 +694,11 @@ Status Engine::batch_step(int32_t* out_slots, int32_t* out_ids, float* out_lps, 
         last_rows_ = rows;
     }
     last_bucket_ = bucket;
+    bool penalised = false;                          // the step with the penalty kernel only when some row needs it
+    for (int r = 0; r < B; ++r) penalised = penalised || slots_[rows[r]].penalised != 0;
     CU(cudaEventRecord(ev_[2], stream_));
-    ST(run_batch_graph(bucket));
+    ST(run_batch_graph(bucket, penalised));
+    const int step_launches = batch_launches_ + (penalised ? 1 : 0) + 1;
     for (int r = 0; r < B; ++r) {                    // sampled rows: the seeded top-k / top-p sampler of the single-sequence path
         const int slot = rows[r];
         if (slots_[slot].sampler == 0) continue;
@@ -653,12 +713,12 @@ Status Engine::batch_step(int32_t* out_slots, int32_t* out_ids, float* out_lps, 
     CU(cudaStreamSynchronize(stream_));
     float step_ms = 0.f;
     cudaEventElapsedTime(&step_ms, ev_[2], ev_[3]);
-    bc_[0] += 1; bc_[1] += (uint64_t)B; bc_[2] += (uint64_t)(step_ms * 1e6); bc_[6] += (uint64_t)batch_launches_ + 1;
+    bc_[0] += 1; bc_[1] += (uint64_t)B; bc_[2] += (uint64_t)(step_ms * 1e6); bc_[6] += (uint64_t)step_launches;
     for (int r = 0; r < B; ++r) {
         SeqSlot& S = slots_[rows[r]];
         S.last_row = r;
         S.eval_ns += (int64_t)(step_ms * 1e6);
-        S.launches += batch_launches_ + 1;
+        S.launches += step_launches;
         if (ho[r].done) {                            // the token just drawn is a stop token: not part of the output
             S.done = true;
             S.stopped = true;
@@ -708,12 +768,12 @@ Status Engine::time_batch_step(int batch, int ctx_len, int iters, float* ms, int
     auto reset = [&]() -> cudaError_t { return cudaMemcpyAsync(bst_, hst.data(), sizeof(StepState) * batch, cudaMemcpyHostToDevice, stream_); };
     CU(reset());
     Status rs;
-    for (int i = 0; i < 3 && rs.ok(); ++i) rs = run_batch_graph(bucket);         // warm-up (captures the bucket's graph)
+    for (int i = 0; i < 3 && rs.ok(); ++i) rs = run_batch_graph(bucket, false);  // warm-up (captures the bucket's graph)
     if (rs.ok()) {
         cudaError_t e = reset();
         if (e == cudaSuccess) e = cudaStreamSynchronize(stream_);                 // hst must outlive the copy
         if (e == cudaSuccess) e = cudaEventRecord(ev_[0], stream_);
-        for (int i = 0; i < iters && rs.ok() && e == cudaSuccess; ++i) rs = run_batch_graph(bucket);
+        for (int i = 0; i < iters && rs.ok() && e == cudaSuccess; ++i) rs = run_batch_graph(bucket, false);
         if (e == cudaSuccess) e = cudaEventRecord(ev_[1], stream_);
         if (e == cudaSuccess) e = cudaEventSynchronize(ev_[1]);
         if (rs.ok() && e != cudaSuccess) rs = failb(GL_ERR_CUDA, std::string("time_batch_step: ") + cudaGetErrorString(e));

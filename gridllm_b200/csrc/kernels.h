@@ -149,6 +149,22 @@ cudaError_t sample_topk_launch(const SampleParams& p, bool fast, bool pdl, cudaS
 // sequential-prefill step without sampling: pos += 1
 cudaError_t advance_launch(StepState* st, bool pdl, cudaStream_t s);
 
+// Repetition / presence / frequency penalties in place on the logits, before the sampler (penalty.cu; semantics in
+// include/gridllm_native.h).  One CTA per row.  History of a row's sequence: prompt[0..st.n_prompt) then out_ids[0..st.out_idx).
+struct BatchCtl;
+struct PenaltyParams {
+    float* logits;          // row r at logits + r * n_vocab
+    int n_vocab;
+    StepState* st;          // ctl == null: the one sequence's state; else [slots]
+    const BatchCtl* ctl;    // batched step: row -> slot, rows >= n_rows leave at once; null: one row, slot 0
+    const int* prompt;      // [slot][prompt_stride]
+    int prompt_stride;
+    const int* out_ids;     // [slot][out_stride]
+    int out_stride;
+    int* counts;            // [slot][n_vocab] int32, zero between launches (each launch leaves it zero)
+};
+cudaError_t penalty_launch(const PenaltyParams& p, int rows, bool pdl, cudaStream_t s);
+
 // standalone pieces (used for fp-weight models and as unfused cross-checks)
 cudaError_t rmsnorm_launch(const float* x, const float* w, int n, float eps, float* y, cudaStream_t s);
 cudaError_t rope_kv_launch(float* q, const float* k, const float* v, int n_head, int n_kv, int head_dim,

@@ -1,7 +1,9 @@
 // Seeded temperature / top-k / top-p sampling of one token from the lm_head logits (InferenceRequest.options.temperature,
 // top_k, top_p, seed: /root/reference/client/src/types/index.ts:1-27; forwarded by OllamaService.generateResponse,
 // /root/reference/client/src/services/OllamaService.ts:101-134).  The arithmetic lives in Ollama in the reference [external];
-// the order followed here is top-k -> temperature -> softmax -> top-p -> inverse-CDF draw, restated in oracle/sampler.py.
+// the order followed here is top-k -> temperature -> softmax -> top-p -> min-p -> inverse-CDF draw, restated in
+// oracle/sampler.py (min-p: tests/penalty_oracle.py).  Repetition penalties (penalty.cu) have already been applied to the
+// logits when a request has them.
 //
 // One CTA of 1024 threads, all passes over the 0.5 MB of logits out of L2:
 //   pass 0   online max / sum of exp (log-softmax of the drawn token at T = 1, the same logprob the greedy sampler reports);
@@ -49,6 +51,13 @@ __device__ __forceinline__ MS ms_merge(MS a, MS b) {
 // ---- the draw itself (one thread): weights in cum[0..k), candidates sorted in cand[0..k) ------------------------------
 __device__ __forceinline__ void draw_and_advance(const SampleParams& p, StepState* st, int out_idx, const unsigned long long* cand, float* cum,
                                                  int k_sel, MS tot) {
+    // min-p: the prefix of candidates whose weight w_j = exp((l_j - l_0) / T) is >= min_p (weights do not increase along the
+    // candidate order, and w_0 = 1, so this is a prefix of at least one); applied after top-p, both cuts are prefixes
+    const float min_p = __ldcg(&st->min_p);
+    int n_minp = k_sel;
+    if (min_p > 0.f)
+        for (int j = 1; j < k_sel; ++j)
+            if (!(cum[j] >= min_p)) { n_minp = j; break; }
     float run = 0.f;
     for (int j = 0; j < k_sel; ++j) { run += cum[j]; cum[j] = run; }
     // top-p: the shortest prefix whose mass reaches top_p of the candidates' mass
@@ -59,6 +68,7 @@ __device__ __forceinline__ void draw_and_advance(const SampleParams& p, StepStat
         for (int j = 0; j < k_sel; ++j)
             if (cum[j] >= lim) { n_keep = j + 1; break; }
     }
+    n_keep = min(n_keep, n_minp);
     // u in [0, 1): 24 bits of splitmix64(seed, output index)
     unsigned long long z = (((unsigned long long)__ldcg(&st->seed_hi) << 32) | __ldcg(&st->seed_lo)) + 0x9E3779B97F4A7C15ull * (unsigned long long)(out_idx + 1);
     z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;

@@ -27,6 +27,7 @@ STATUS_NAMES = {0: "GL_OK", -1: "GL_ERR_INVALID", -2: "GL_ERR_IO", -3: "GL_ERR_F
 ABI_SYMBOLS = [
     "gl_abi_version", "gl_last_error", "gl_device_count", "gl_engine_create", "gl_engine_destroy",
     "gl_engine_info", "gl_tokenize", "gl_detokenize", "gl_chat_template", "gl_generate", "gl_embed", "gl_last_logits", "gl_sample_logits",
+    "gl_penalize_logits",
     "gl_seq_open", "gl_seq_open_many", "gl_batch_step", "gl_seq_close", "gl_seq_logits", "gl_seq_stats", "gl_token_piece", "gl_token_text", "gl_batch_counters", "gl_time_batch_step",
     "gl_gemv", "gl_gemv_model_tensor", "gl_rmsnorm", "gl_decode_step", "gl_kv_reset", "gl_position",
     "gl_prefill", "gl_time_decode",
@@ -59,7 +60,20 @@ class ModelInfo(C.Structure):
 class SampleOpts(C.Structure):
     _fields_ = [("num_predict", C.c_int32), ("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float),
                 ("seed", C.c_uint64), ("ignore_eos", C.c_int32), ("n_stop_ids", C.c_int32),
-                ("stop_ids", C.POINTER(C.c_int32)), ("want_logits", C.c_int32), ("reserved", C.c_int32 * 6)]
+                ("stop_ids", C.POINTER(C.c_int32)), ("want_logits", C.c_int32),
+                # repetition penalties and min_p (include/gridllm_native.h); zero = off
+                ("repeat_penalty", C.c_float), ("repeat_last_n", C.c_int32), ("presence_penalty", C.c_float),
+                ("frequency_penalty", C.c_float), ("min_p", C.c_float), ("reserved", C.c_int32 * 1)]
+
+# the keywords of generate / seq_open / seq_open_many / sample_logits that fill the fields above, with values that mean "off"
+# (repeat_last_n 64 is Ollama's default window: setting only repeat_penalty penalises the last 64 ids, as Ollama does)
+PENALTY_DEFAULTS = {"repeat_penalty": 1.0, "repeat_last_n": 64, "presence_penalty": 0.0, "frequency_penalty": 0.0, "min_p": 0.0}
+
+
+def _set_penalties(so: SampleOpts, kw: dict) -> None:
+    v = dict(PENALTY_DEFAULTS, **{k: x for k, x in kw.items() if x is not None})
+    so.repeat_penalty, so.repeat_last_n = float(v["repeat_penalty"]), int(v["repeat_last_n"])
+    so.presence_penalty, so.frequency_penalty, so.min_p = float(v["presence_penalty"]), float(v["frequency_penalty"]), float(v["min_p"])
 
 
 class GenStats(C.Structure):
@@ -98,6 +112,7 @@ def load_library() -> C.CDLL:
     lib.gl_embed.argtypes = [vp, i32p, i32p, i32, f32p, C.POINTER(GenStats)]
     lib.gl_last_logits.argtypes = [vp, i32, f32p, i32]
     lib.gl_sample_logits.argtypes = [vp, f32p, i32, C.POINTER(SampleOpts), i32, i32p, f32p]
+    lib.gl_penalize_logits.argtypes = [vp, f32p, i32, C.POINTER(SampleOpts), i32p, i32]
     lib.gl_seq_open.argtypes = [vp, i32p, i32, C.POINTER(SampleOpts), i32p]
     lib.gl_seq_open_many.argtypes = [vp, i32p, i32p, i32, C.POINTER(SampleOpts), i32p, i32p]
     lib.gl_batch_step.argtypes = [vp, i32p, i32p, f32p, i32p, i32, i32p]
@@ -206,11 +221,14 @@ class Engine:
     def generate(self, prompt: Sequence[int], num_predict: int = 128, ignore_eos: bool = False,
                  on_token: Optional[Callable[[int, float, bytes], bool]] = None, want_logits: bool = False,
                  stop_ids: Sequence[int] = (), temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0,
-                 seed: int = 0) -> Generation:
+                 seed: int = 0, repeat_penalty: float = 1.0, repeat_last_n: int = 64, presence_penalty: float = 0.0,
+                 frequency_penalty: float = 0.0, min_p: float = 0.0) -> Generation:
         p = np.ascontiguousarray(prompt, dtype=np.int32)
         so = SampleOpts()
         so.num_predict, so.ignore_eos, so.want_logits = num_predict, int(ignore_eos), int(want_logits)
         so.temperature, so.top_k, so.top_p, so.seed = float(temperature), int(top_k), float(top_p), int(seed) & (2**64 - 1)
+        _set_penalties(so, dict(repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n, presence_penalty=presence_penalty,
+                                frequency_penalty=frequency_penalty, min_p=min_p))
         stops = np.ascontiguousarray(stop_ids, dtype=np.int32)
         so.n_stop_ids = len(stops)
         so.stop_ids = _i32p(stops) if len(stops) else None
@@ -234,11 +252,14 @@ class Engine:
 
     # ---- continuous batching (gl_seq_open / gl_batch_step / gl_seq_close) ---------------------------------
     def seq_open(self, prompt: Sequence[int], num_predict: int = 128, ignore_eos: bool = False, temperature: float = 0.0, top_k: int = 0,
-                 top_p: float = 1.0, seed: int = 0, stop_ids: Sequence[int] = ()) -> int:
+                 top_p: float = 1.0, seed: int = 0, stop_ids: Sequence[int] = (), repeat_penalty: float = 1.0, repeat_last_n: int = 64,
+                 presence_penalty: float = 0.0, frequency_penalty: float = 0.0, min_p: float = 0.0) -> int:
         p = np.ascontiguousarray(prompt, dtype=np.int32)
         so = SampleOpts()
         so.num_predict, so.ignore_eos = (num_predict if num_predict > 0 else 128), int(ignore_eos)
         so.temperature, so.top_k, so.top_p, so.seed = float(temperature), int(top_k), float(top_p), int(seed) & (2**64 - 1)
+        _set_penalties(so, dict(repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n, presence_penalty=presence_penalty,
+                                frequency_penalty=frequency_penalty, min_p=min_p))
         stops = np.ascontiguousarray(stop_ids, dtype=np.int32)
         so.n_stop_ids = len(stops)
         so.stop_ids = _i32p(stops) if len(stops) else None
@@ -261,6 +282,7 @@ class Engine:
             so[i].num_predict, so[i].ignore_eos = (np_ if np_ > 0 else 128), int(bool(o.get("ignore_eos", False)))
             so[i].temperature, so[i].top_k, so[i].top_p = float(o.get("temperature", 0.0)), int(o.get("top_k", 0)), float(o.get("top_p", 1.0))
             so[i].seed = int(o.get("seed", 0)) & (2**64 - 1)
+            _set_penalties(so[i], {k: o.get(k) for k in PENALTY_DEFAULTS})
             stops = np.ascontiguousarray(o.get("stop_ids", ()), dtype=np.int32)
             keep.append(stops)
             so[i].n_stop_ids = len(stops)
@@ -319,15 +341,29 @@ class Engine:
         return ms.value, nl.value, wb.value
 
     def sample_logits(self, logits: np.ndarray, temperature: float, top_k: int = 0, top_p: float = 1.0, seed: int = 0,
-                      out_index: int = 0):
+                      out_index: int = 0, min_p: float = 0.0):
         """The sampler alone (gl_sample_logits): (token id, logprob) for output number out_index of such a request."""
         a = np.ascontiguousarray(logits, dtype=np.float32)
         so = SampleOpts()
         so.num_predict, so.ignore_eos = 1, 1
         so.temperature, so.top_k, so.top_p, so.seed = float(temperature), int(top_k), float(top_p), int(seed) & (2**64 - 1)
+        _set_penalties(so, dict(min_p=min_p))
         tid, lp = C.c_int32(0), C.c_float(0.0)
         _check(self._lib.gl_sample_logits(self._h, _f32p(a), len(a), C.byref(so), out_index, C.byref(tid), C.byref(lp)))
         return int(tid.value), float(lp.value)
+
+    def penalize_logits(self, logits: np.ndarray, history: Sequence[int], repeat_penalty: float = 1.0, repeat_last_n: int = 64,
+                        presence_penalty: float = 0.0, frequency_penalty: float = 0.0) -> np.ndarray:
+        """The repetition-penalty kernel alone (gl_penalize_logits): a penalised copy of `logits` for a sequence whose history
+        (prompt ids, then generated ids) is `history`."""
+        out = np.array(logits, dtype=np.float32, copy=True)
+        h = np.ascontiguousarray(history, dtype=np.int32)
+        so = SampleOpts()
+        so.num_predict, so.ignore_eos = 1, 1
+        _set_penalties(so, dict(repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n, presence_penalty=presence_penalty,
+                                frequency_penalty=frequency_penalty))
+        _check(self._lib.gl_penalize_logits(self._h, _f32p(out), len(out), C.byref(so), _i32p(h) if len(h) else None, len(h)))
+        return out
 
     def last_logits(self, step: int) -> np.ndarray:
         out = np.empty(self.info.n_vocab, dtype=np.float32)

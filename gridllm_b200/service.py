@@ -86,10 +86,13 @@ class NativeInferenceService:
 
     # what Ollama applies when a request leaves the sampling options out [external: Ollama's documented parameter defaults]
     OLLAMA_SAMPLING_DEFAULTS = {"temperature": 0.8, "top_k": 40, "top_p": 0.9}
+    # Ollama's defaults for the repetition penalty [external: Ollama's documented parameter defaults]; opt-in, like the dict above
+    OLLAMA_PENALTY_DEFAULTS = {"repeat_penalty": 1.1, "repeat_last_n": 64}
+    PENALTY_OPTIONS = ("repeat_penalty", "repeat_last_n", "presence_penalty", "frequency_penalty", "min_p")
 
     def __init__(self, models: Dict[str, str], device: int = 0, max_ctx: int = 0,
                  sampling_defaults: Optional[Dict[str, Any]] = None, apply_template: bool = False, max_batch: int = 0,
-                 jinja_templates: bool = True, **engine_kw):
+                 jinja_templates: bool = True, penalty_defaults: Optional[Dict[str, Any]] = None, **engine_kw):
         """models: Ollama-style model name -> GGUF path.
         sampling_defaults: options a request inherits when it does not carry them.  None = greedy (temperature 0, the
         BASELINE.json configuration); pass OLLAMA_SAMPLING_DEFAULTS to behave like an Ollama worker for such requests.
@@ -97,8 +100,11 @@ class NativeInferenceService:
         metadata.system as the system turn) unless metadata.raw, as Ollama does; default False = raw prompts.
         max_batch: > 1 turns on continuous batching (SURVEY.md section 8f.1): concurrent generate* calls become sequences of
         one engine and are decoded together, one batched step per token (gridllm_b200/batching.py); 0 / 1 = one request at a time.
-        jinja_templates: render tokenizer.chat_template as Jinja for chat requests (default); False = family framing only."""
+        jinja_templates: render tokenizer.chat_template as Jinja for chat requests (default); False = family framing only.
+        penalty_defaults: repetition-penalty options a request inherits when it does not carry them.  None = no penalty; pass
+        OLLAMA_PENALTY_DEFAULTS to penalise like an Ollama worker."""
         self._sampling_defaults = dict(sampling_defaults or {})
+        self._penalty_defaults = dict(penalty_defaults or {})
         # Ollama wraps the prompt of /api/generate and /v1/completions in the model's template (system + prompt as one user
         # turn) unless the request says raw [external]; off by default: the prompt text is tokenised as it is
         self._apply_template = bool(apply_template)
@@ -321,7 +327,7 @@ class NativeInferenceService:
 
     def _plan(self, eng: N.Engine, ids: np.ndarray, num_predict: int, options: Dict[str, Any], on_token):
         """-> (num_predict, ignore_eos, sampling kw, token callback, finish(gen)): what one generation needs, however it is run"""
-        kw = self._sampling(options)
+        kw = dict(self._sampling(options), **self._penalties(options))
         ignore_eos = bool(options.get("ignore_eos", False))
         # a generation that would run past the engine's context ends at it (done_reason "length") instead of failing; a prompt
         # that does not fit at all still fails (GL_ERR_CONTEXT)
@@ -393,6 +399,43 @@ class NativeInferenceService:
         if seed is None:
             seed = secrets.randbits(63)
         return {"temperature": temperature, "top_k": top_k, "top_p": top_p, "seed": int(seed)}
+
+    def _penalties(self, options: Dict[str, Any]) -> Dict[str, Any]:
+        """InferenceRequest.options.{repeat_penalty, repeat_last_n, presence_penalty, frequency_penalty, min_p} (validated by the
+        gateway, server/src/routes/ollama.ts:26-39; the OpenAI routes map frequency_penalty / presence_penalty onto the same
+        keys, openai.ts:406-410) -> the engine's penalty keywords.  {} when the request sets none of them.  A request that sets a
+        penalty but no window gets Ollama's window of 64.  Out-of-range values fail the request, as a bad temperature does."""
+        defaults = getattr(self, "_penalty_defaults", {})
+
+        def opt(name):
+            v = options.get(name)
+            return defaults.get(name) if v is None else v
+        given = {k: opt(k) for k in self.PENALTY_OPTIONS if opt(k) is not None}
+        if not given:
+            return {}
+        out: Dict[str, Any] = {}
+        for k, v in given.items():
+            if isinstance(v, bool):
+                raise RuntimeError(f"{k} must be a number")
+            try:
+                f = float(v)
+            except (TypeError, ValueError):
+                raise RuntimeError(f"{k} must be a number")
+            if not np.isfinite(f):
+                raise RuntimeError(f"{k} must be a finite number")
+            if k == "repeat_last_n":
+                if f != int(f) or f < -1:
+                    raise RuntimeError("repeat_last_n must be an integer >= -1")
+                out[k] = int(f)
+            else:
+                out[k] = f
+        if out.get("repeat_penalty", 0.0) < 0:
+            raise RuntimeError("repeat_penalty must be >= 0")
+        if not 0.0 <= out.get("min_p", 0.0) <= 1.0:
+            raise RuntimeError("min_p must lie in [0, 1]")
+        if "repeat_last_n" not in out and any(k in out for k in ("repeat_penalty", "presence_penalty", "frequency_penalty")):
+            out["repeat_last_n"] = 64
+        return out
 
     def _response(self, request: InferenceRequest, eng: N.Engine, gen: N.Generation, text: str) -> InferenceResponse:
         st = gen.stats

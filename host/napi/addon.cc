@@ -83,6 +83,18 @@ napi_value CreateEngine(napi_env env, napi_callback_info info) {
     return ext;
 }
 
+// repetition penalties and min_p (Ollama's options of the same names, camel-cased like the other sampling options); an absent
+// property leaves the field at its zero, which means "off" (include/gridllm_native.h)
+void read_penalty_opts(napi_env env, napi_value o, gl_sample_opts& so) {
+    napi_value v;
+    double d = 0.0;
+    if (napi_get_named_property(env, o, "repeatPenalty", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.repeat_penalty = (float)d;
+    if (napi_get_named_property(env, o, "repeatLastN", &v) == napi_ok) napi_get_value_int32(env, v, &so.repeat_last_n);
+    if (napi_get_named_property(env, o, "presencePenalty", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.presence_penalty = (float)d;
+    if (napi_get_named_property(env, o, "frequencyPenalty", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.frequency_penalty = (float)d;
+    if (napi_get_named_property(env, o, "minP", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.min_p = (float)d;
+}
+
 // ---- generate: async work + threadsafe token callback --------------------------------------------------
 struct GenJob {
     gl_engine* e;
@@ -192,6 +204,7 @@ napi_value Generate(napi_env env, napi_callback_info info) {
     if (napi_get_named_property(env, argv[2], "topP", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) j->so.top_p = (float)d;
     bool lossless = false;
     if (napi_get_named_property(env, argv[2], "seed", &v) == napi_ok) napi_get_value_bigint_uint64(env, v, &j->so.seed, &lossless);
+    read_penalty_opts(env, argv[2], j->so);
     napi_valuetype vt;
     if (argc > 3 && napi_typeof(env, argv[3], &vt) == napi_ok && vt == napi_function) {
         napi_value name;
@@ -378,6 +391,7 @@ void read_sample_opts(napi_env env, napi_value o, gl_sample_opts& so, std::vecto
     if (napi_get_named_property(env, o, "topK", &v) == napi_ok) napi_get_value_int32(env, v, &so.top_k);
     if (napi_get_named_property(env, o, "topP", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.top_p = (float)d;
     if (napi_get_named_property(env, o, "seed", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.seed = (uint64_t)d;
+    read_penalty_opts(env, o, so);
     if (napi_get_named_property(env, o, "stopIds", &v) == napi_ok) {
         void* data; size_t n; napi_typedarray_type ty; napi_value ab; size_t off;
         if (napi_get_typedarray_info(env, v, &ty, &n, &data, &ab, &off) == napi_ok && ty == napi_int32_array)

@@ -151,7 +151,33 @@ export class NativeInferenceService {
 		if (numPredict < 0) numPredict = nCtx > 0 ? Math.max(1, nCtx - nPrompt) : 128;
 		if (nCtx > 0 && nPrompt < nCtx) numPredict = Math.min(numPredict, nCtx - nPrompt);
 		return { numPredict, ignoreEos: !!o.ignore_eos, temperature, topK: o.top_k ?? d.top_k ?? 0, topP: o.top_p ?? d.top_p ?? 1,
-			seed: BigInt(o.seed ?? (temperature > 0 ? Math.floor(Math.random() * 2 ** 53) : 0)) };
+			seed: BigInt(o.seed ?? (temperature > 0 ? Math.floor(Math.random() * 2 ** 53) : 0)), ...this.penaltyOpts(o) };
+	}
+
+	// GRIDLLM_PENALTIES=ollama: requests that leave the repetition penalty out inherit Ollama's defaults (repeat_penalty 1.1 over
+	// the last 64 ids); default: no penalty.  Same mapping as gridllm_b200/service.py::_penalties.
+	private penaltyDefaults: Record<string, number> = process.env.GRIDLLM_PENALTIES === "ollama" ? { repeat_penalty: 1.1, repeat_last_n: 64 } : {};
+
+	// options.{repeat_penalty, repeat_last_n, presence_penalty, frequency_penalty, min_p} (gateway: ollama.ts:26-39; the OpenAI
+	// routes use the same keys) -> the addon's penalty fields.  Absent: none of them (the engine's zeros mean "off").  A penalty
+	// without a window gets Ollama's window of 64.
+	private penaltyOpts(o: Record<string, any>) {
+		const d = this.penaltyDefaults;
+		const pick = (k: string): number | undefined => (o[k] ?? d[k]);
+		const out: Record<string, number> = {};
+		for (const [k, name] of [["repeat_penalty", "repeatPenalty"], ["repeat_last_n", "repeatLastN"], ["presence_penalty", "presencePenalty"],
+			["frequency_penalty", "frequencyPenalty"], ["min_p", "minP"]] as const) {
+			const v = pick(k);
+			if (v === undefined || v === null) continue;
+			if (typeof v !== "number" || !Number.isFinite(v)) throw new Error(`${k} must be a finite number`);
+			out[name] = v;
+		}
+		if (out.repeatPenalty !== undefined && out.repeatPenalty < 0) throw new Error("repeat_penalty must be >= 0");
+		if (out.repeatLastN !== undefined && (!Number.isInteger(out.repeatLastN) || out.repeatLastN < -1)) throw new Error("repeat_last_n must be an integer >= -1");
+		if (out.minP !== undefined && !(out.minP >= 0 && out.minP <= 1)) throw new Error("min_p must lie in [0, 1]");
+		if (out.repeatLastN === undefined && (out.repeatPenalty !== undefined || out.presencePenalty !== undefined || out.frequencyPenalty !== undefined))
+			out.repeatLastN = 64;
+		return out;
 	}
 
 	async generateResponse(request: InferenceRequest): Promise<InferenceResponse> {   // :97-184

@@ -87,7 +87,23 @@ typedef struct gl_sample_opts {
     int32_t  n_stop_ids;
     const int32_t* stop_ids;  /* extra stop token ids (host resolves stop strings) */
     int32_t  want_logits;     /* 1: keep per-step logits for gl_last_logits (parity tests) */
-    int32_t  reserved[6];
+    /* Repetition penalties (Ollama's options of the same names; arithmetic of llama.cpp's penalties sampler, which Ollama's
+     * runner uses -- parity with a real Ollama is unpinned, like the sampler's).  A caller that zeroes these fields gets no
+     * penalty and no min_p: every field's zero means "off".
+     * History H of a sequence = the prompt ids of the call (BOS and any prepended context included), then every token generated
+     * so far (a drawn stop token ends the sequence and is never added).  Window W = the last N entries of H: N = repeat_last_n
+     * when > 0, the whole of H when -1; 0 turns every penalty off.  Before EVERY draw (the first token after the prompt
+     * included; greedy and sampled alike), for each distinct id t in W occurring c times, in single fp32 operations:
+     *   a = logit[t];  if repeat_penalty is active (> 0 and != 1): a = a <= 0 ? a * repeat_penalty : a / repeat_penalty;
+     *   logit[t] = a - (c * frequency_penalty + presence_penalty).
+     * Reported logprobs and the logits of gl_last_logits / gl_seq_logits are those of the PENALISED logits (what the token was
+     * drawn from).  Invalid (GL_ERR_INVALID): non-finite values, repeat_penalty < 0, repeat_last_n < -1, min_p outside [0, 1]. */
+    float    repeat_penalty;    /* 0 or 1: off */
+    int32_t  repeat_last_n;     /* window: > 0 last N ids, -1 the whole history, 0 no penalty of any kind */
+    float    presence_penalty;  /* subtracted once from every id in the window */
+    float    frequency_penalty; /* subtracted once per occurrence in the window */
+    float    min_p;             /* temperature > 0 only: after top-p keep the prefix of candidates with exp((l - l0) / T) >= min_p; 0 = off */
+    int32_t  reserved[1];
 } gl_sample_opts;
 
 typedef struct gl_gen_stats {
@@ -146,7 +162,8 @@ int  gl_embed(gl_engine* e, const int32_t* ids, const int32_t* seq_offsets, int3
  *                 the token drawn was a stop token (not part of the output).  Finished sequences stay open, holding
  *                 their pages, until gl_seq_close.  *n = entries written (<= cap).
  *   gl_seq_close  return the slot and its pages.
- *   gl_seq_logits logits [n_vocab] the sequence's LAST token was drawn from (parity tests; valid until the next step).
+ *   gl_seq_logits logits [n_vocab] the sequence's LAST token was drawn from, penalties applied (parity tests; valid until the
+ *                 next step).
  * Sequences join and leave between steps; a sequence's tokens do not depend on who shares its batch. */
 int  gl_seq_open(gl_engine* e, const int32_t* prompt, int32_t n_prompt, const gl_sample_opts* opts, int32_t* slot);
 /* Several prompts in one call: they share one packed prompt pass (block-diagonal causal attention, every weight matrix read
@@ -178,14 +195,22 @@ int  gl_batch_counters(gl_engine* e, uint64_t out[8], int32_t reset);
 int  gl_time_batch_step(gl_engine* e, int32_t batch, int32_t ctx_len, int32_t iters, float* ms_per_step, int32_t* launches_per_step,
                         uint64_t* weight_bytes);
 
-/* logits of generation step i of the last gl_generate that ran with want_logits=1 */
+/* logits of generation step i of the last gl_generate that ran with want_logits=1 (after the repetition penalties, if the
+ * request had any: the logits the token was drawn from) */
 int  gl_last_logits(gl_engine* e, int32_t step, float* out, int32_t n_vocab);
 
 /* the sampler alone on caller-supplied logits [n_vocab]: the token gl_generate would emit as output number out_index
- * of a request with these options (temperature 0: argmax; else the seeded top-k / top-p draw), and its log-softmax.
- * Parity tests of the draw against oracle/sampler.py.  Rewinds the sequence like gl_kv_reset(). */
+ * of a request with these options (temperature 0: argmax; else the seeded top-k / top-p / min-p draw), and its log-softmax.
+ * No repetition penalty is applied (see gl_penalize_logits).  Parity tests of the draw against oracle/sampler.py (min-p: tests/penalty_oracle.py).  Rewinds
+ * the sequence like gl_kv_reset(). */
 int  gl_sample_logits(gl_engine* e, const float* logits, int32_t n_vocab, const gl_sample_opts* opts, int32_t out_index,
                       int32_t* id, float* logprob);
+/* the repetition-penalty kernel alone, in place on caller-supplied logits [n_vocab], with history[0..n_history) as the
+ * sequence's history H (the penalty fields of opts; everything else in opts is ignored).  Parity tests against
+ * tests/penalty_oracle.py; hosts may probe for this symbol to learn that the penalty fields are honoured.  Rewinds the sequence
+ * like gl_kv_reset(). */
+int  gl_penalize_logits(gl_engine* e, float* logits, int32_t n_vocab, const gl_sample_opts* opts, const int32_t* history,
+                        int32_t n_history);
 
 /* ---- kernel-level entry points (parity tests and roofline measurement) ------------------ */
 /* y[rows] = W[rows x cols] (GGUF-layout blocks of ggml_type, host memory) * x[cols].
