@@ -47,6 +47,16 @@ const char* check_penalties(const gl_sample_opts& so) {
     if (so.min_p < 0.f || so.min_p > 1.f) return "min_p must lie in [0, 1]";
     return nullptr;
 }
+
+// format took the place of the last reserved word (an anonymous union keeps `reserved` addressable): a zeroed word is "off"
+static_assert(offsetof(gl_sample_opts, format) == 64, "format sits where reserved[0] was");
+
+// the format field of a generating request; nullptr when valid
+const char* check_format(const gl_sample_opts& so) {
+    if (so.format != 0 && so.format != GL_FORMAT_JSON) return "format must be 0 (off) or GL_FORMAT_JSON";
+    if (so.format == GL_FORMAT_JSON && so.ignore_eos) return "format json cannot be combined with ignore_eos: a JSON document ends on a stop token";
+    return nullptr;
+}
 }  // namespace
 
 extern "C" {
@@ -139,6 +149,7 @@ int gl_generate(gl_engine* e, const int32_t* prompt, int32_t n_prompt, const gl_
     if (opts) so = *opts;
     else { so.num_predict = 128; so.top_p = 1.f; }
     if (const char* m = check_penalties(so)) return bad(m);
+    if (const char* m = check_format(so)) return bad(m);
     return ret(e->impl->generate(prompt, n_prompt, so, cb, user, out_ids, out_logprobs, stats));
 }
 
@@ -154,6 +165,7 @@ int gl_seq_open(gl_engine* e, const int32_t* prompt, int32_t n_prompt, const gl_
     if (opts) so = *opts;
     else { so.num_predict = 128; so.top_p = 1.f; }
     if (const char* m = check_penalties(so)) return bad(m);
+    if (const char* m = check_format(so)) return bad(m);
     int s = -1;
     const int rc = ret(e->impl->seq_open(prompt, n_prompt, so, &s));
     if (rc == GL_OK) *slot = s;
@@ -163,8 +175,10 @@ int gl_seq_open(gl_engine* e, const int32_t* prompt, int32_t n_prompt, const gl_
 int gl_seq_open_many(gl_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seq, const gl_sample_opts* opts, int32_t* slots,
                      int32_t* n_opened) {
     if (!e || !ids || !offsets || !opts || !slots || !n_opened) return bad("gl_seq_open_many: null argument");
-    for (int32_t i = 0; i < n_seq; ++i)
+    for (int32_t i = 0; i < n_seq; ++i) {
         if (const char* m = check_penalties(opts[i])) return bad(m);
+        if (const char* m = check_format(opts[i])) return bad(m);
+    }
     int k = 0;
     const int rc = ret(e->impl->seq_open_many(ids, offsets, n_seq, opts, slots, &k));
     *n_opened = k;
@@ -249,6 +263,13 @@ int gl_penalize_logits(gl_engine* e, float* logits, int32_t n_vocab, const gl_sa
     if (!e || !logits || !opts) return bad("gl_penalize_logits: null argument");
     if (const char* m = check_penalties(*opts)) return bad(m);
     return ret(e->impl->penalize_logits(logits, n_vocab, *opts, history, n_history));
+}
+
+int gl_constrain_logits(gl_engine* e, float* logits, int32_t n_vocab, const gl_sample_opts* opts, const int32_t* generated,
+                        int32_t n_generated) {
+    if (!e || !logits || !opts) return bad("gl_constrain_logits: null argument");
+    if (opts->format != 0 && opts->format != GL_FORMAT_JSON) return bad("format must be 0 (off) or GL_FORMAT_JSON");
+    return ret(e->impl->constrain_logits(logits, n_vocab, *opts, generated, n_generated));
 }
 
 int gl_gemv(gl_engine* e, int ggml_type, const void* w_host, int32_t rows, int32_t cols, const float* x, float* y, int32_t iters,

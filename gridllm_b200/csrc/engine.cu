@@ -11,6 +11,7 @@
 #include <thread>
 
 #include "common.cuh"
+#include "json_fsm.h"
 #include "rowdot.h"
 
 namespace gl {
@@ -80,8 +81,9 @@ Engine::~Engine() {
     if (g_nohead_) cudaGraphExecDestroy(g_nohead_);
     for (auto& v : g_head_var_)
         for (auto& k : v)
-            for (auto& g : k)
-                if (g) cudaGraphExecDestroy(g);
+            for (auto& j : k)
+                for (auto& g : j)
+                    if (g) cudaGraphExecDestroy(g);
     for (auto& v : g_batch_)
         for (auto& g : v)
             if (g) cudaGraphExecDestroy(g);
@@ -456,11 +458,14 @@ StepState Engine::make_state(int pos, int token, int n_prompt, int out_idx, cons
     h.presence_penalty = pen ? so->presence_penalty : 0.f;
     h.frequency_penalty = pen ? so->frequency_penalty : 0.f;
     if (penalised) *penalised = pen ? 1 : 0;
+    // JSON grammar mask (json_mask.cu): json_st starts zeroed, the automaton's initial state
+    h.json = (so && so->format == GL_FORMAT_JSON) ? 1 : 0;
     return h;
 }
 
 Status Engine::set_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so) {
     const StepState h = make_state(pos, token, n_prompt, out_idx, so, &sampler_, &penalised_);
+    json_ = h.json;
     if (bar_counter_) CU(cudaMemsetAsync(bar_counter_, 0, 4, stream_));
     CU(cudaMemcpyAsync(st_, &h, sizeof(h), cudaMemcpyHostToDevice, stream_));
     CU(cudaStreamSynchronize(stream_));     // h is on the stack
@@ -621,6 +626,11 @@ Status Engine::enqueue_head(cudaStream_t s, bool keep_logits, int* n_launch) {
         CU(penalty_launch(pp, 1, false, s));
         ++*n_launch;
     }
+    if (json_) {               // the JSON grammar mask after the penalties, right before the draw (json_mask.cu)
+        JsonMaskParams jp{logits_, n_vocab_, st_, nullptr, json_off_, json_bytes_, json_cls_};
+        CU(json_mask_launch(jp, 1, false, s));
+        ++*n_launch;
+    }
     SampleParams sp{logits_, n_vocab_, st_, out_ids_, out_lp_, keep_logits ? logits_keep_ : nullptr, keep_logits ? keep_cap_ : max_out_, sample_scratch_, topk_scratch_};
     if (sampler_ != 0) CU(sample_topk_launch(sp, sampler_ == 1, pdl && fused_ && sampler_pdl_, s));      // temperature > 0: seeded top-k / top-p draw (sampler.cu)
     else CU(sample_greedy_launch(sp, pdl && fused_ && greedy_pdl_, s));
@@ -641,7 +651,7 @@ Status Engine::build_graphs() {
         e = cudaGraphInstantiate(&ge, g, 0);
         cudaGraphDestroy(g);
         if (e != cudaSuccess) return fail(GL_ERR_CUDA, std::string("graph instantiate: ") + cudaGetErrorString(e));
-        if (which == 0) { g_nohead_ = ge; launches_nohead_ = n; } else { g_head_var_[0][0][0] = ge; launches_head_ = n; }
+        if (which == 0) { g_nohead_ = ge; launches_nohead_ = n; } else { g_head_var_[0][0][0][0] = ge; launches_head_ = n; }
     }
     return {};
 }
@@ -653,9 +663,9 @@ Status Engine::run_steps(int n_nohead, int n_head, bool keep_logits) {
         if (n_head > 0) ST(launch_mega(n_head, true, keep_logits));
         return {};
     }
-    // the step with a head exists in twelve captured variants (sampler x plain / logits kept x without / with the penalty
-    // kernel); all but the first lazily
-    cudaGraphExec_t* head = &g_head_var_[sampler_][keep_logits ? 1 : 0][penalised_ ? 1 : 0];
+    // the step with a head exists in 24 captured variants (sampler x plain / logits kept x without / with the penalty kernel x
+    // without / with the JSON mask kernel); all but the first lazily
+    cudaGraphExec_t* head = &g_head_var_[sampler_][keep_logits ? 1 : 0][penalised_ ? 1 : 0][json_ ? 1 : 0];
     if (use_graph_ && n_head > 0 && !*head) {
         cudaGraph_t g = nullptr;
         CU(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
@@ -804,6 +814,7 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
         make_state(0, 0, n_prompt, 0, &so, nullptr, &pen);
         if (pen) return fail(GL_ERR_UNSUPPORTED, "the persistent decode kernel (GL_MEGA=1) has no repetition penalties");
     }
+    ST(json_admit(so, true));
     for (int i = 0; i < n_prompt; ++i)
         if (prompt[i] < 0 || prompt[i] >= n_vocab_) return fail(GL_ERR_INVALID, "prompt token id out of range");
     ST(kv_reset());
@@ -816,8 +827,9 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
             logits_keep_ = p;
             keep_cap_ = n_pred;
             for (auto& v : g_head_var_)
-                for (auto& g : v[1])
-                    if (g) { cudaGraphExecDestroy(g); g = nullptr; }      // captured with the old logits buffer
+                for (auto& k : v[1])
+                    for (auto& g : k)
+                        if (g) { cudaGraphExecDestroy(g); g = nullptr; }      // captured with the old logits buffer
         }
     }
     CU(cudaMemcpyAsync(prompt_ids_, prompt, (size_t)n_prompt * 4, cudaMemcpyHostToDevice, stream_));
@@ -951,6 +963,139 @@ Status Engine::penalize_logits(float* logits, int n_vocab, const gl_sample_opts&
         if (ce == cudaSuccess) ce = cudaMemcpyAsync(logits, logits_, (size_t)n_vocab_ * 4, cudaMemcpyDeviceToHost, stream_);
         if (ce == cudaSuccess) ce = cudaStreamSynchronize(stream_);
         if (ce != cudaSuccess) rs = fail(GL_ERR_CUDA, std::string("penalize_logits: ") + cudaGetErrorString(ce));
+    } while (false);
+    if (hist) cudaFree(hist);
+    ST(rs);
+    return kv_reset();
+}
+
+// ---- JSON grammar mask (json_mask.cu) --------------------------------------------------------------------------------
+// The vocabulary table the mask kernel reads, built once at the first JSON request.  The vocabulary must guarantee that every
+// state the automaton can reach has an allowed token, so that the mask never leaves a draw with nothing: a single-byte piece for
+// each of \t, \n and 0x20-0x7E (all of them ordinary tokens, not stop tokens), one for each of 0x80-0xBF as soon as some piece
+// is not whole well-formed UTF-8 (a string can then stop inside a character), and an eos token to end on.
+Status Engine::ensure_json() {
+    if (json_checked_) return json_refused_.empty() ? Status{} : fail(GL_ERR_UNSUPPORTED, json_refused_);
+    json_checked_ = true;
+    if (!tok_.ok()) json_refused_ = "format json: the model carries no tokenizer";
+    else if (tok_.eos < 0) json_refused_ = "format json: the vocabulary has no eos token to end a document on";
+    if (!json_refused_.empty()) return fail(GL_ERR_UNSUPPORTED, json_refused_);
+    std::vector<uint32_t> off(n_vocab_ + 1, 0);
+    std::vector<uint8_t> bytes, cls(n_vocab_, 0);
+    bool single[256] = {};
+    bool partial_utf8 = false;
+    for (int t = 0; t < n_vocab_; ++t) {
+        const std::string pc = tok_.piece(t);
+        off[t] = (uint32_t)bytes.size();
+        bytes.insert(bytes.end(), pc.begin(), pc.end());
+        bool plain = !pc.empty();
+        for (unsigned char c : pc) plain = plain && c >= 0x20 && c <= 0x7E && c != '"' && c != '\\';
+        cls[t] = plain ? JSON_CLS_PLAIN : 0;
+        if (pc.size() == 1 && t != tok_.eos && t != tok_.eot) single[(unsigned char)pc[0]] = true;
+        // whole well-formed UTF-8?  (the string-body automaton from its own state accepts it and ends outside a character)
+        JsonState u{};
+        u.mode = JM_STR;
+        bool whole = true;
+        for (unsigned char c : pc)      // (quotes, backslashes and control bytes stand in for one plain character here)
+            if (!json_step(u, (c == '"' || c == '\\' || c < 0x20) ? (uint8_t)'a' : (uint8_t)c)) { whole = false; break; }
+        if (!whole || u.mode != JM_STR) partial_utf8 = true;
+    }
+    off[n_vocab_] = (uint32_t)bytes.size();
+    std::string missing;
+    auto need = [&](int b) {
+        if (!single[b]) {
+            char buf[8];
+            snprintf(buf, sizeof buf, "0x%02X", b);
+            missing += (missing.empty() ? "" : ", ") + std::string(buf);
+        }
+    };
+    need('\t');
+    need('\n');
+    for (int b = 0x20; b <= 0x7E; ++b) need(b);
+    if (partial_utf8)
+        for (int b = 0x80; b <= 0xBF; ++b) need(b);
+    if (!missing.empty()) {
+        json_refused_ = "format json: the vocabulary has no single-byte token for byte(s) " + missing +
+                        ", so a JSON continuation cannot be guaranteed";
+        return fail(GL_ERR_UNSUPPORTED, json_refused_);
+    }
+    uint32_t* d_off = nullptr;
+    uint8_t *d_bytes = nullptr, *d_cls = nullptr;
+    CU(cudaMalloc((void**)&d_off, off.size() * 4));
+    allocs_.push_back(d_off);
+    CU(cudaMalloc((void**)&d_bytes, std::max<size_t>(bytes.size(), 1)));
+    allocs_.push_back(d_bytes);
+    CU(cudaMalloc((void**)&d_cls, cls.size()));
+    allocs_.push_back(d_cls);
+    CU(cudaMemcpy(d_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    if (!bytes.empty()) CU(cudaMemcpy(d_bytes, bytes.data(), bytes.size(), cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_cls, cls.data(), cls.size(), cudaMemcpyHostToDevice));
+    json_off_ = d_off; json_bytes_ = d_bytes; json_cls_ = d_cls;
+    json_hoff_ = std::move(off);
+    json_hbytes_ = std::move(bytes);
+    return {};
+}
+
+bool Engine::json_stop(const gl_sample_opts& so, int32_t id) const {
+    const StepState h = make_state(0, 0, 0, 0, &so, nullptr);      // the stop ids the device sees
+    for (int k = 0; k < h.n_stop; ++k)
+        if (h.stop_ids[k] == id) return true;
+    return false;
+}
+
+Status Engine::json_admit(const gl_sample_opts& so, bool single_path) {
+    if (so.format == 0) return {};
+    if (so.format != GL_FORMAT_JSON) return fail(GL_ERR_INVALID, "format must be 0 (off) or GL_FORMAT_JSON");
+    if (so.ignore_eos) return fail(GL_ERR_INVALID, "format json cannot be combined with ignore_eos: a JSON document ends on a stop token");
+    if (single_path && use_mega_) return fail(GL_ERR_UNSUPPORTED, "the persistent decode kernel (GL_MEGA=1) has no JSON grammar mask");
+    ST(ensure_json());
+    // a stop id that is an ordinary token would be masked wherever it is needed, and the vocabulary guarantee would not hold
+    for (int i = 0; i < so.n_stop_ids; ++i) {
+        const int32_t id = so.stop_ids ? so.stop_ids[i] : -1;
+        if (id >= 0 && id < n_vocab_ && json_hoff_[id + 1] != json_hoff_[id])
+            return fail(GL_ERR_INVALID, "format json: stop_ids must be control tokens (empty piece); use stop strings for text");
+    }
+    return {};
+}
+
+// The automaton through a caller-supplied output history, then the mask kernel alone on caller-supplied logits (parity tests
+// against tests/json_oracle.py).  Rewinds the sequence.
+Status Engine::constrain_logits(float* logits, int n_vocab, const gl_sample_opts& so, const int32_t* generated, int n_generated) {
+    CU(cudaSetDevice(device_));
+    if (!logits || n_vocab != n_vocab_) return fail(GL_ERR_INVALID, "logits must hold n_vocab values");
+    if (n_generated < 0 || (n_generated > 0 && !generated)) return fail(GL_ERR_INVALID, "bad history");
+    if (n_generated >= max_out_) return fail(GL_ERR_INVALID, "history longer than an output");
+    for (int i = 0; i < n_generated; ++i)
+        if (generated[i] < 0 || generated[i] >= n_vocab_) return fail(GL_ERR_INVALID, "history token id out of range");
+    gl_sample_opts o = so;
+    o.ignore_eos = 0;
+    if (o.format == 0) return {};                      // off: the logits stay as they are
+    ST(json_admit(o, false));
+    // the history must be a prefix the mask allows: no stop token (it would have ended the output), no control token, every
+    // byte accepted
+    JsonState hs{};
+    for (int i = 0; i < n_generated; ++i) {
+        const int32_t t = generated[i];
+        const uint32_t a = json_hoff_[t], b = json_hoff_[t + 1];
+        if (json_stop(o, t) || a == b || !json_run(hs, json_hbytes_.data() + a, (int)(b - a)))
+            return fail(GL_ERR_INVALID, "format json: the history is not a prefix the grammar allows (token " + std::to_string(i) + ")");
+    }
+    ST(kv_reset());
+    ST(set_state(0, n_generated > 0 ? generated[n_generated - 1] : 0, 0, n_generated, &o));
+    int* hist = nullptr;
+    if (n_generated > 0) CU(cudaMalloc((void**)&hist, (size_t)n_generated * 4));
+    Status rs;
+    do {
+        cudaError_t ce = hist ? cudaMemcpyAsync(hist, generated, (size_t)n_generated * 4, cudaMemcpyHostToDevice, stream_) : cudaSuccess;
+        if (ce == cudaSuccess && hist) ce = json_replay_launch(st_, hist, n_generated, json_off_, json_bytes_, stream_);
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(logits_, logits, (size_t)n_vocab_ * 4, cudaMemcpyHostToDevice, stream_);
+        if (ce == cudaSuccess) {
+            JsonMaskParams jp{logits_, n_vocab_, st_, nullptr, json_off_, json_bytes_, json_cls_};
+            ce = json_mask_launch(jp, 1, false, stream_);
+        }
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(logits, logits_, (size_t)n_vocab_ * 4, cudaMemcpyDeviceToHost, stream_);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(stream_);
+        if (ce != cudaSuccess) rs = fail(GL_ERR_CUDA, std::string("constrain_logits: ") + cudaGetErrorString(ce));
     } while (false);
     if (hist) cudaFree(hist);
     ST(rs);

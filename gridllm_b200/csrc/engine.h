@@ -71,6 +71,7 @@ public:
     Status time_batch_step(int batch, int ctx_len, int iters, float* ms, int* launches, uint64_t* wbytes);
     Status sample_logits(const float* logits, int n_vocab, const gl_sample_opts& so, int out_index, int* id, float* logprob);
     Status penalize_logits(float* logits, int n_vocab, const gl_sample_opts& so, const int32_t* history, int n_history);
+    Status constrain_logits(float* logits, int n_vocab, const gl_sample_opts& so, const int32_t* generated, int n_generated);
     Status gemv_host(int type, const void* w_host, int rows, int cols, const float* x, float* y, int iters, float* ms);
     Status gemv_tensor(const std::string& name, const float* x, float* y, int iters, int flush, float* ms, uint64_t* wbytes);
     Status rmsnorm(const float* x, const float* w, int n, float eps, float* y);
@@ -199,7 +200,7 @@ private:
     struct SeqSlot {
         bool open = false, done = false, first_pending = false;
         std::vector<int> pages;
-        int n_prompt = 0, n_pred = 0, produced = 0, sampler = 0, penalised = 0;
+        int n_prompt = 0, n_pred = 0, produced = 0, sampler = 0, penalised = 0, json = 0;
         int32_t last_token = 0;
         float first_lp = 0.f;
         int last_row = -1;                            // row of the last batched step this sequence took part in
@@ -236,29 +237,46 @@ private:
     std::string qg_why_not_;                          // why the quantised path is unavailable for this model (message for batch_weights = 2)
     Status build_qgemm_weights();
     Status pack_qgemm(const std::vector<const GGUFTensor*>& src, int mode, QGemmWeights& out, uint8_t*& tmp, size_t& tmp_cap);
-    cudaGraphExec_t g_batch_[N_BUCKETS][2] = {};      // [bucket][1: with the penalty kernel, for steps in which some row has penalties]
-    int batch_launches_ = 0;                          // kernels of one batched step (without the penalty kernel)
+    // [bucket][variant]: variant bit 0 the penalty kernel (steps in which some row has penalties), bit 1 the JSON mask kernel
+    // (steps in which some row has format json)
+    cudaGraphExec_t g_batch_[N_BUCKETS][4] = {};
+    int batch_launches_ = 0;                          // kernels of one batched step (without the penalty / JSON mask kernels)
     uint64_t bc_[8] = {};                             // gl_batch_counters
     Status ensure_batch_state();
     Status seq_open_single(const int32_t* prompt, int n_prompt, const gl_sample_opts& so, int* slot);
-    Status enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, int* n_launch);
-    Status run_batch_graph(int bucket, bool penalised);
+    Status enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bool json, int* n_launch);
+    Status run_batch_graph(int bucket, bool penalised, bool json);
     cudaError_t batch_penalty_launch(int bucket, cudaStream_t s);
+    cudaError_t batch_json_launch(int bucket, cudaStream_t s);
+    bool batch_json_checked_ = false;                 // the batched mask launch has run once outside stream capture
     Status ensure_batch_penalty();                    // bprompt_ / bpen_counts_, allocated when the first penalised sequence opens
     Status keep_prompt(int slot, const int32_t* prompt, int n_prompt);     // a penalised slot's prompt -> bprompt_
     static int bucket_of(int rows) { int b = 8; while (b < rows) b <<= 1; return b; }
     static int bucket_index(int bucket) { int i = 0; while ((8 << i) < bucket) ++i; return i; }
 
     cudaGraphExec_t g_nohead_ = nullptr;
-    cudaGraphExec_t g_head_var_[3][2][2] = {};   // [sampler of the running request][logits kept][repetition penalties]
+    cudaGraphExec_t g_head_var_[3][2][2][2] = {};   // [sampler of the running request][logits kept][repetition penalties][format json]
     int penalised_ = 0;                        // the running request has penalties: penalty.cu runs between the lm_head and the sampler
+    int json_ = 0;                             // the running request has format json: json_mask.cu runs right before the sampler
+    // JSON grammar mask (json_mask.cu): the vocabulary's pieces on the device, built at the first JSON request (nothing before)
+    uint32_t* json_off_ = nullptr;             // [n_vocab + 1] byte offsets
+    uint8_t* json_bytes_ = nullptr;            // pieces back to back
+    uint8_t* json_cls_ = nullptr;              // [n_vocab] JSON_CLS_* bits
+    std::vector<uint32_t> json_hoff_;          // host copies (history validation of gl_constrain_logits)
+    std::vector<uint8_t> json_hbytes_;
+    bool json_checked_ = false;
+    std::string json_refused_;                 // why this model cannot take JSON requests ("" once the table is built)
+    Status ensure_json();
+    // a request's format field: GL_ERR_UNSUPPORTED / GL_ERR_INVALID when the engine cannot honour it (table built on first use)
+    Status json_admit(const gl_sample_opts& so, bool single_path);
+    bool json_stop(const gl_sample_opts& so, int32_t id) const;     // id is a stop token of a request with these options
     // The top-k samplers are launched WITHOUT programmatic dependent launch: their CTAs (33 KB of shared memory each) resident
     // beside the lm_head CTAs cost the step 60 us (run 67: 1.537 -> 1.478 ms/token at top_k 40); the greedy sampler keeps it.
     bool sampler_pdl_ = false;
     bool greedy_pdl_ = false;                 // the greedy sampler likewise (64 small CTAs: 3 us per token, run 68)
     int sampler_ = 0;                          // 0 greedy (argmax), 1 / 2: the two kernels of sampler.cu (temperature > 0)
     int launches_nohead_ = 0, launches_head_ = 0;    // launches_head_: the step with a head WITHOUT the penalty kernel
-    int head_launches() const { return launches_head_ + (penalised_ && !use_mega_ ? 1 : 0); }     // ... of the variant that runs
+    int head_launches() const { return launches_head_ + (use_mega_ ? 0 : (penalised_ ? 1 : 0) + (json_ ? 1 : 0)); }     // ... of the variant that runs
     cudaEvent_t ev_[4] = {nullptr, nullptr, nullptr, nullptr};
     int64_t load_ns_ = 0;
     uint64_t weight_bytes_ = 0, decode_bytes_ = 0, n_params_ = 0;

@@ -180,7 +180,7 @@ Status Engine::ensure_batch_state() {
     // launch configuration is validated -- and every lazily initialised driver entry point touched -- OUTSIDE stream capture,
     // where an error has a name
     int nl = 0;
-    ST(enqueue_batch_step(stream_, 8, false, &nl));
+    ST(enqueue_batch_step(stream_, 8, false, false, &nl));
     CU(cudaStreamSynchronize(stream_));
     batch_launches_ = nl;
     batch_ready_ = true;
@@ -216,6 +216,13 @@ cudaError_t Engine::batch_penalty_launch(int bucket, cudaStream_t s) {
     return penalty_launch(pp, bucket, false, s);
 }
 
+// the JSON grammar mask over the rows of a batched step (row r: logits row r, the state of slot row_slot[r]; rows without JSON
+// leave at once)
+cudaError_t Engine::batch_json_launch(int bucket, cudaStream_t s) {
+    JsonMaskParams jp{blogits_, n_vocab_, bst_, bctl_, json_off_, json_bytes_, json_cls_};
+    return json_mask_launch(jp, bucket, false, s);
+}
+
 // Prefill a prompt into a free slot's own pages and draw its first token.  The single-sequence code runs unchanged on the
 // slot's state: the members it reads (page table, step state, output buffers) point at the slot's rows for the duration.
 // One prompt.  It takes the SAME path as a prompt opened together with others (gl_seq_open_many with one entry: packed prompt
@@ -240,6 +247,7 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
     for (int i = 0; i < n_prompt; ++i)
         if (prompt[i] < 0 || prompt[i] >= n_vocab_) return failb(GL_ERR_INVALID, "prompt token id out of range");
     if (!(so.temperature >= 0.f) || !std::isfinite(so.temperature)) return failb(GL_ERR_INVALID, "temperature must be a finite number >= 0");
+    ST(json_admit(so, false));
     ST(ensure_batch_state());
     const int n_pred = so.num_predict > 0 ? so.num_predict : 128;
     if (n_prompt + n_pred > n_ctx_) return failb(GL_ERR_CONTEXT, "prompt + num_predict exceeds the engine context");
@@ -308,6 +316,7 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
     }
     S.open = true;
     S.n_prompt = n_prompt; S.n_pred = n_pred; S.produced = 0; S.sampler = sampler; S.penalised = penalised; S.first_pending = true;
+    S.json = so.format == GL_FORMAT_JSON ? 1 : 0;
     S.t_open_ns = t_open; S.launches = prefill_launches; S.stopped = S.done;
     bc_[3] += (uint64_t)S.prefill_ns; bc_[4] += (uint64_t)n_prompt; bc_[5] += 1; bc_[6] += (uint64_t)prefill_launches;
     *slot_out = slot;
@@ -333,6 +342,7 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
         if (!(opts[i].temperature >= 0.f) || !std::isfinite(opts[i].temperature)) return failb(GL_ERR_INVALID, "temperature must be a finite number >= 0");
         const int n_pred = opts[i].num_predict > 0 ? opts[i].num_predict : 128;
         if (n + n_pred > n_ctx_) return failb(GL_ERR_CONTEXT, "prompt + num_predict exceeds the engine context");
+        ST(json_admit(opts[i], false));
     }
     if (!pk_ids_) {
         auto dalloc = [&](void** p, size_t bytes) -> cudaError_t {
@@ -416,13 +426,15 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             std::vector<StepState> hst(P);
             BatchCtl hc{};
             hc.n_rows = P;
-            bool any_pen = false;
+            bool any_pen = false, any_json = false;
             for (int i = 0; i < P && ce == cudaSuccess; ++i) {
                 const int w = which[i], n = lens[i];
                 int sampler = 0, pen = 0;
                 hst[i] = make_state(n - 1, ids[offs[w] + n - 1], n, 0, &opts[w], &sampler, &pen);
                 slots_[pslots[i]].sampler = sampler;
                 slots_[pslots[i]].penalised = pen;
+                slots_[pslots[i]].json = hst[i].json;
+                any_json = any_json || hst[i].json != 0;
                 if (pen) {                                   // the head of the history the penalty kernel reads
                     Status ks = keep_prompt(pslots[i], ids + offs[w], n);
                     if (!ks.ok()) { rs = ks; break; }
@@ -437,6 +449,10 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             const int bucket = bucket_of(P);
             if (ce == cudaSuccess && any_pen) {              // penalties before every first-token draw of the pack
                 ce = batch_penalty_launch(bucket, stream_);
+                ++launches;
+            }
+            if (ce == cudaSuccess && any_json) {             // then the JSON grammar mask of the rows that have it
+                ce = batch_json_launch(bucket, stream_);
                 ++launches;
             }
             if (ce == cudaSuccess) ce = batch_sample_greedy_launch(blogits_, n_vocab_, bucket, bctl_, bst_, bout_ids_, bout_lp_, max_out_, bsample_scratch_, stream_);
@@ -530,7 +546,7 @@ Status Engine::seq_logits(int slot, float* out, int n_vocab) {
 }
 
 // every launch of one batched step, for `bucket` rows; all pointers are fixed, the composition is read from bctl_ / bst_
-Status Engine::enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, int* n_launch) {
+Status Engine::enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bool json, int* n_launch) {
     const int qd = n_head_ * hd_, kvd = n_kv_ * hd_, ldq = qd + 2 * kvd;
     const float scale = 1.0f / std::sqrt((float)hd_);
     int nl = 0;
@@ -614,34 +630,55 @@ Status Engine::enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, in
     // repetition penalties of the rows that have them (penalty.cu), before every sampler of the step: only in the variant used
     // for steps in which some row has penalties
     if (penalised) { CU(batch_penalty_launch(bucket, s)); ++nl; }
+    // then the JSON grammar mask of the rows that have format json (json_mask.cu): only in the variants used for steps in which
+    // some row has it
+    if (json) { CU(batch_json_launch(bucket, s)); ++nl; }
     CU(batch_sample_greedy_launch(blogits_, n_vocab_, bucket, bctl_, bst_, bout_ids_, bout_lp_, max_out_, bsample_scratch_, s)); ++nl;
     if (n_launch) *n_launch = nl;
     return {};
 }
 
-// penalised: the variant with the penalty kernel (a second captured step per bucket); batch_launches_ counts the plain one
-Status Engine::run_batch_graph(int bucket, bool penalised) {
+// penalised / json: the variants with the penalty kernel / the JSON mask kernel (up to four captured steps per bucket);
+// batch_launches_ counts the plain one
+Status Engine::run_batch_graph(int bucket, bool penalised, bool json) {
     const int bi = bucket_index(bucket);
     if (penalised && !bpen_counts_) return failb(GL_ERR_INVALID, "batched step: no penalty state");
+    if (json && !json_off_) return failb(GL_ERR_INVALID, "batched step: no JSON vocabulary table");
+    const int extra = (penalised ? 1 : 0) + (json ? 1 : 0);
     if (!use_graph_) {
         int nl = 0;
-        ST(enqueue_batch_step(stream_, bucket, penalised, &nl));
-        batch_launches_ = nl - (penalised ? 1 : 0);
+        ST(enqueue_batch_step(stream_, bucket, penalised, json, &nl));
+        batch_launches_ = nl - extra;
         return {};
     }
-    cudaGraphExec_t& ge = g_batch_[bi][penalised ? 1 : 0];
+    cudaGraphExec_t& ge = g_batch_[bi][(penalised ? 1 : 0) | (json ? 2 : 0)];
     if (!ge) {
+        if (json && !batch_json_checked_) {
+            // one un-captured launch on a composition of no rows (every CTA leaves at once; a launch on the real rows would
+            // advance their automata) validates the configuration outside stream capture; the step's composition is restored
+            BatchCtl none{};
+            CU(cudaMemcpyAsync(bctl_, &none, sizeof(int), cudaMemcpyHostToDevice, stream_));
+            cudaError_t e0 = batch_json_launch(8, stream_);
+            if (e0 == cudaSuccess) e0 = cudaStreamSynchronize(stream_);
+            BatchCtl h{};
+            h.n_rows = (int)last_rows_.size();
+            for (int r = 0; r < h.n_rows; ++r) h.row_slot[r] = last_rows_[r];
+            CU(cudaMemcpyAsync(bctl_, &h, sizeof(h), cudaMemcpyHostToDevice, stream_));
+            CU(cudaStreamSynchronize(stream_));                       // h is on the stack
+            CU(e0);
+            batch_json_checked_ = true;
+        }
         cudaGraph_t g = nullptr;
         int nl = 0;
         CU(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
-        Status st = enqueue_batch_step(stream_, bucket, penalised, &nl);
+        Status st = enqueue_batch_step(stream_, bucket, penalised, json, &nl);
         cudaError_t e = cudaStreamEndCapture(stream_, &g);
         if (!st.ok()) { if (g) cudaGraphDestroy(g); return st; }
         if (e != cudaSuccess) return failb(GL_ERR_CUDA, std::string("batched step: graph capture: ") + cudaGetErrorString(e));
         e = cudaGraphInstantiate(&ge, g, 0);
         cudaGraphDestroy(g);
         if (e != cudaSuccess) return failb(GL_ERR_CUDA, std::string("batched step: graph instantiate: ") + cudaGetErrorString(e));
-        batch_launches_ = nl - (penalised ? 1 : 0);
+        batch_launches_ = nl - extra;
     }
     CU(cudaGraphLaunch(ge, stream_));
     return {};
@@ -694,11 +731,14 @@ Status Engine::batch_step(int32_t* out_slots, int32_t* out_ids, float* out_lps, 
         last_rows_ = rows;
     }
     last_bucket_ = bucket;
-    bool penalised = false;                          // the step with the penalty kernel only when some row needs it
-    for (int r = 0; r < B; ++r) penalised = penalised || slots_[rows[r]].penalised != 0;
+    bool penalised = false, json = false;            // the step with the penalty / JSON mask kernel only when some row needs it
+    for (int r = 0; r < B; ++r) {
+        penalised = penalised || slots_[rows[r]].penalised != 0;
+        json = json || slots_[rows[r]].json != 0;
+    }
     CU(cudaEventRecord(ev_[2], stream_));
-    ST(run_batch_graph(bucket, penalised));
-    const int step_launches = batch_launches_ + (penalised ? 1 : 0) + 1;
+    ST(run_batch_graph(bucket, penalised, json));
+    const int step_launches = batch_launches_ + (penalised ? 1 : 0) + (json ? 1 : 0) + 1;
     for (int r = 0; r < B; ++r) {                    // sampled rows: the seeded top-k / top-p sampler of the single-sequence path
         const int slot = rows[r];
         if (slots_[slot].sampler == 0) continue;
@@ -768,12 +808,12 @@ Status Engine::time_batch_step(int batch, int ctx_len, int iters, float* ms, int
     auto reset = [&]() -> cudaError_t { return cudaMemcpyAsync(bst_, hst.data(), sizeof(StepState) * batch, cudaMemcpyHostToDevice, stream_); };
     CU(reset());
     Status rs;
-    for (int i = 0; i < 3 && rs.ok(); ++i) rs = run_batch_graph(bucket, false);  // warm-up (captures the bucket's graph)
+    for (int i = 0; i < 3 && rs.ok(); ++i) rs = run_batch_graph(bucket, false, false);  // warm-up (captures the bucket's graph)
     if (rs.ok()) {
         cudaError_t e = reset();
         if (e == cudaSuccess) e = cudaStreamSynchronize(stream_);                 // hst must outlive the copy
         if (e == cudaSuccess) e = cudaEventRecord(ev_[0], stream_);
-        for (int i = 0; i < iters && rs.ok() && e == cudaSuccess; ++i) rs = run_batch_graph(bucket, false);
+        for (int i = 0; i < iters && rs.ok() && e == cudaSuccess; ++i) rs = run_batch_graph(bucket, false, false);
         if (e == cudaSuccess) e = cudaEventRecord(ev_[1], stream_);
         if (e == cudaSuccess) e = cudaEventSynchronize(ev_[1]);
         if (rs.ok() && e != cudaSuccess) rs = failb(GL_ERR_CUDA, std::string("time_batch_step: ") + cudaGetErrorString(e));

@@ -165,6 +165,23 @@ struct PenaltyParams {
 };
 cudaError_t penalty_launch(const PenaltyParams& p, int rows, bool pdl, cudaStream_t s);
 
+// JSON grammar mask in place on the logits, after the penalties and before the sampler (json_mask.cu; language in json_fsm.h,
+// semantics in include/gridllm_native.h).  Grid: vocabulary chunks x rows, one thread per token.  A row's automaton state
+// lives in its StepState (json_st, two entries by output-index parity); rows without JSON and finished rows leave at once.
+struct JsonMaskParams {
+    float* logits;              // row r at logits + r * n_vocab
+    int n_vocab;
+    StepState* st;              // ctl == null: the one sequence's state; else [slots]
+    const BatchCtl* ctl;        // batched step: row -> slot, rows >= n_rows leave at once; null: one row, slot 0
+    const uint32_t* offsets;    // [n_vocab + 1] byte offsets of the token pieces
+    const uint8_t* bytes;       // the pieces, back to back
+    const uint8_t* cls;         // [n_vocab] class bits (JSON_CLS_*)
+};
+cudaError_t json_mask_launch(const JsonMaskParams& p, int rows, bool pdl, cudaStream_t s);
+// one thread: the automaton from the initial state through the pieces of ids[0..n-1) (all but the last), stored as the entry
+// the mask kernel of output n reads; that kernel then advances by ids[n-1] (= st->token) itself.  gl_constrain_logits.
+cudaError_t json_replay_launch(StepState* st, const int* ids, int n, const uint32_t* offsets, const uint8_t* bytes, cudaStream_t s);
+
 // standalone pieces (used for fp-weight models and as unfused cross-checks)
 cudaError_t rmsnorm_launch(const float* x, const float* w, int n, float eps, float* y, cudaStream_t s);
 cudaError_t rope_kv_launch(float* q, const float* k, const float* v, int n_head, int n_kv, int head_dim,

@@ -27,7 +27,7 @@ STATUS_NAMES = {0: "GL_OK", -1: "GL_ERR_INVALID", -2: "GL_ERR_IO", -3: "GL_ERR_F
 ABI_SYMBOLS = [
     "gl_abi_version", "gl_last_error", "gl_device_count", "gl_engine_create", "gl_engine_destroy",
     "gl_engine_info", "gl_tokenize", "gl_detokenize", "gl_chat_template", "gl_generate", "gl_embed", "gl_last_logits", "gl_sample_logits",
-    "gl_penalize_logits",
+    "gl_penalize_logits", "gl_constrain_logits",
     "gl_seq_open", "gl_seq_open_many", "gl_batch_step", "gl_seq_close", "gl_seq_logits", "gl_seq_stats", "gl_token_piece", "gl_token_text", "gl_batch_counters", "gl_time_batch_step",
     "gl_gemv", "gl_gemv_model_tensor", "gl_rmsnorm", "gl_decode_step", "gl_kv_reset", "gl_position",
     "gl_prefill", "gl_time_decode",
@@ -57,13 +57,32 @@ class ModelInfo(C.Structure):
                 ("decode_bytes_per_token", C.c_uint64), ("device", C.c_int32), ("sm_count", C.c_int32)]
 
 
+class _FormatWord(C.Union):
+    _fields_ = [("format", C.c_int32), ("reserved", C.c_int32 * 1)]
+
+
 class SampleOpts(C.Structure):
+    _anonymous_ = ("_fmt",)
     _fields_ = [("num_predict", C.c_int32), ("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float),
                 ("seed", C.c_uint64), ("ignore_eos", C.c_int32), ("n_stop_ids", C.c_int32),
                 ("stop_ids", C.POINTER(C.c_int32)), ("want_logits", C.c_int32),
                 # repetition penalties and min_p (include/gridllm_native.h); zero = off
                 ("repeat_penalty", C.c_float), ("repeat_last_n", C.c_int32), ("presence_penalty", C.c_float),
-                ("frequency_penalty", C.c_float), ("min_p", C.c_float), ("reserved", C.c_int32 * 1)]
+                ("frequency_penalty", C.c_float), ("min_p", C.c_float),
+                # output format (0 off, GL_FORMAT_JSON), in the union with the last reserved word
+                ("_fmt", _FormatWord)]
+
+
+GL_FORMAT_JSON = 1
+
+
+def _format_code(fmt) -> int:
+    """the `format` keyword -> gl_sample_opts.format: None / "" / 0 off, "json" (or GL_FORMAT_JSON) the JSON grammar mask"""
+    if fmt is None or fmt == "" or fmt == 0:
+        return 0
+    if fmt == "json" or fmt == GL_FORMAT_JSON:
+        return GL_FORMAT_JSON
+    raise ValueError(f"format must be None or 'json', not {fmt!r}")
 
 # the keywords of generate / seq_open / seq_open_many / sample_logits that fill the fields above, with values that mean "off"
 # (repeat_last_n 64 is Ollama's default window: setting only repeat_penalty penalises the last 64 ids, as Ollama does)
@@ -113,6 +132,7 @@ def load_library() -> C.CDLL:
     lib.gl_last_logits.argtypes = [vp, i32, f32p, i32]
     lib.gl_sample_logits.argtypes = [vp, f32p, i32, C.POINTER(SampleOpts), i32, i32p, f32p]
     lib.gl_penalize_logits.argtypes = [vp, f32p, i32, C.POINTER(SampleOpts), i32p, i32]
+    lib.gl_constrain_logits.argtypes = [vp, f32p, i32, C.POINTER(SampleOpts), i32p, i32]
     lib.gl_seq_open.argtypes = [vp, i32p, i32, C.POINTER(SampleOpts), i32p]
     lib.gl_seq_open_many.argtypes = [vp, i32p, i32p, i32, C.POINTER(SampleOpts), i32p, i32p]
     lib.gl_batch_step.argtypes = [vp, i32p, i32p, f32p, i32p, i32, i32p]
@@ -222,10 +242,11 @@ class Engine:
                  on_token: Optional[Callable[[int, float, bytes], bool]] = None, want_logits: bool = False,
                  stop_ids: Sequence[int] = (), temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0,
                  seed: int = 0, repeat_penalty: float = 1.0, repeat_last_n: int = 64, presence_penalty: float = 0.0,
-                 frequency_penalty: float = 0.0, min_p: float = 0.0) -> Generation:
+                 frequency_penalty: float = 0.0, min_p: float = 0.0, format: Optional[str] = None) -> Generation:
         p = np.ascontiguousarray(prompt, dtype=np.int32)
         so = SampleOpts()
         so.num_predict, so.ignore_eos, so.want_logits = num_predict, int(ignore_eos), int(want_logits)
+        so.format = _format_code(format)
         so.temperature, so.top_k, so.top_p, so.seed = float(temperature), int(top_k), float(top_p), int(seed) & (2**64 - 1)
         _set_penalties(so, dict(repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n, presence_penalty=presence_penalty,
                                 frequency_penalty=frequency_penalty, min_p=min_p))
@@ -253,10 +274,11 @@ class Engine:
     # ---- continuous batching (gl_seq_open / gl_batch_step / gl_seq_close) ---------------------------------
     def seq_open(self, prompt: Sequence[int], num_predict: int = 128, ignore_eos: bool = False, temperature: float = 0.0, top_k: int = 0,
                  top_p: float = 1.0, seed: int = 0, stop_ids: Sequence[int] = (), repeat_penalty: float = 1.0, repeat_last_n: int = 64,
-                 presence_penalty: float = 0.0, frequency_penalty: float = 0.0, min_p: float = 0.0) -> int:
+                 presence_penalty: float = 0.0, frequency_penalty: float = 0.0, min_p: float = 0.0, format: Optional[str] = None) -> int:
         p = np.ascontiguousarray(prompt, dtype=np.int32)
         so = SampleOpts()
         so.num_predict, so.ignore_eos = (num_predict if num_predict > 0 else 128), int(ignore_eos)
+        so.format = _format_code(format)
         so.temperature, so.top_k, so.top_p, so.seed = float(temperature), int(top_k), float(top_p), int(seed) & (2**64 - 1)
         _set_penalties(so, dict(repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n, presence_penalty=presence_penalty,
                                 frequency_penalty=frequency_penalty, min_p=min_p))
@@ -283,6 +305,7 @@ class Engine:
             so[i].temperature, so[i].top_k, so[i].top_p = float(o.get("temperature", 0.0)), int(o.get("top_k", 0)), float(o.get("top_p", 1.0))
             so[i].seed = int(o.get("seed", 0)) & (2**64 - 1)
             _set_penalties(so[i], {k: o.get(k) for k in PENALTY_DEFAULTS})
+            so[i].format = _format_code(o.get("format"))
             stops = np.ascontiguousarray(o.get("stop_ids", ()), dtype=np.int32)
             keep.append(stops)
             so[i].n_stop_ids = len(stops)
@@ -363,6 +386,21 @@ class Engine:
         _set_penalties(so, dict(repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n, presence_penalty=presence_penalty,
                                 frequency_penalty=frequency_penalty))
         _check(self._lib.gl_penalize_logits(self._h, _f32p(out), len(out), C.byref(so), _i32p(h) if len(h) else None, len(h)))
+        return out
+
+    def constrain_logits(self, logits: np.ndarray, generated: Sequence[int], format: Optional[str] = "json",
+                         stop_ids: Sequence[int] = ()) -> np.ndarray:
+        """The JSON grammar mask alone (gl_constrain_logits): a masked copy of `logits` for the draw that follows the output
+        `generated` (token ids after the prompt).  NativeError GL_ERR_INVALID when `generated` is not a prefix the mask allows."""
+        out = np.array(logits, dtype=np.float32, copy=True)
+        g = np.ascontiguousarray(generated, dtype=np.int32)
+        so = SampleOpts()
+        so.num_predict = 1
+        so.format = _format_code(format)
+        stops = np.ascontiguousarray(stop_ids, dtype=np.int32)
+        so.n_stop_ids = len(stops)
+        so.stop_ids = _i32p(stops) if len(stops) else None
+        _check(self._lib.gl_constrain_logits(self._h, _f32p(out), len(out), C.byref(so), _i32p(g) if len(g) else None, len(g)))
         return out
 
     def last_logits(self, step: int) -> np.ndarray:

@@ -325,10 +325,13 @@ class NativeInferenceService:
     def _stop_ids(self, eng: N.Engine, request: InferenceRequest) -> List[int]:
         return []
 
-    def _plan(self, eng: N.Engine, ids: np.ndarray, num_predict: int, options: Dict[str, Any], on_token):
-        """-> (num_predict, ignore_eos, sampling kw, token callback, finish(gen)): what one generation needs, however it is run"""
-        kw = dict(self._sampling(options), **self._penalties(options))
+    def _plan(self, eng: N.Engine, ids: np.ndarray, num_predict: int, options: Dict[str, Any], on_token, fmt=None):
+        """-> (num_predict, ignore_eos, sampling kw, token callback, finish(gen)): what one generation needs, however it is run.
+        fmt: the request's _format keywords ({} / None: free text)."""
+        kw = dict(self._sampling(options), **self._penalties(options), **(fmt or {}))
         ignore_eos = bool(options.get("ignore_eos", False))
+        if fmt and ignore_eos:
+            raise RuntimeError("format json cannot be combined with ignore_eos: a JSON document ends on a stop token")
         # a generation that would run past the engine's context ends at it (done_reason "length") instead of failing; a prompt
         # that does not fit at all still fails (GL_ERR_CONTEXT)
         n_ctx = int(getattr(eng.info, "n_ctx", 0) or 0)
@@ -361,22 +364,22 @@ class NativeInferenceService:
             return gen
         return num_predict, ignore_eos, kw, cb, finish
 
-    def _run(self, model: str, ids: np.ndarray, num_predict: int, options: Dict[str, Any], on_token=None):
+    def _run(self, model: str, ids: np.ndarray, num_predict: int, options: Dict[str, Any], on_token=None, fmt=None):
         """one request at a time: the blocking gl_generate call (runs on a worker thread)"""
         eng = self._engine(model)
-        num_predict, ignore_eos, kw, cb, finish = self._plan(eng, ids, num_predict, options, on_token)
+        num_predict, ignore_eos, kw, cb, finish = self._plan(eng, ids, num_predict, options, on_token, fmt)
         with self._lock:
             gen = eng.generate(ids, num_predict=num_predict, ignore_eos=ignore_eos, on_token=cb, **kw)
         return eng, finish(gen)
 
-    async def _generate(self, model: str, ids: np.ndarray, num_predict: int, options: Dict[str, Any], on_token=None):
+    async def _generate(self, model: str, ids: np.ndarray, num_predict: int, options: Dict[str, Any], on_token=None, fmt=None):
         """-> (engine, Generation).  With continuous batching the request becomes a sequence of the engine's batch runner and
         this coroutine just awaits its future (no thread is parked per request: 256 concurrent jobs are 256 futures); otherwise
         the blocking call runs on a worker thread.  Either way the event loop stays free for heartbeats."""
         if not self._max_batch:
-            return await asyncio.to_thread(self._run, model, ids, num_predict, options, on_token)
+            return await asyncio.to_thread(self._run, model, ids, num_predict, options, on_token, fmt)
         eng = await self._engine_async(model)
-        num_predict, ignore_eos, kw, cb, finish = self._plan(eng, ids, num_predict, options, on_token)
+        num_predict, ignore_eos, kw, cb, finish = self._plan(eng, ids, num_predict, options, on_token, fmt)
         runner = await asyncio.to_thread(self._runner, model)
         gen = await asyncio.wrap_future(runner.submit(ids, num_predict, ignore_eos, kw, cb))
         return eng, finish(gen)
@@ -437,6 +440,22 @@ class NativeInferenceService:
             out["repeat_last_n"] = 64
         return out
 
+    @staticmethod
+    def _format(request: InferenceRequest) -> Dict[str, Any]:
+        """The request's output format -> the engine's `format` keyword.  metadata.format first (the gateway's Ollama routes,
+        server/src/routes/ollama.ts:229, 385), then options.format (its OpenAI route, openai.ts:636-642).  "json" turns the
+        JSON grammar mask on; so does a JSON-schema object, but the schema itself is NOT enforced (the response is valid JSON of
+        any shape).  Absent, None or "" is free text ({}); anything else fails the request, as a bad temperature does."""
+        md = request.get("metadata") or {}
+        fmt = md.get("format")
+        if fmt is None or fmt == "":
+            fmt = (request.get("options") or {}).get("format")
+        if fmt is None or fmt == "":
+            return {}
+        if fmt == "json" or isinstance(fmt, dict):
+            return {"format": "json"}
+        raise RuntimeError(f'format must be "json" or a JSON schema object, not {fmt!r}')
+
     def _response(self, request: InferenceRequest, eng: N.Engine, gen: N.Generation, text: str) -> InferenceResponse:
         st = gen.stats
         if getattr(gen, "stop_text", None) is not None:      # options.stop was active: the filtered text is the response
@@ -470,9 +489,10 @@ class NativeInferenceService:
         try:
             options = request.get("options") or {}
             num_predict = self._num_predict(options)
+            fmt = self._format(request)
             eng = await self._engine_async(request["model"])
             ids = self._prompt_ids(eng, request, request.get("prompt"))
-            eng, gen = await self._generate(request["model"], ids, num_predict, options)
+            eng, gen = await self._generate(request["model"], ids, num_predict, options, fmt=fmt)
             return self._response(request, eng, gen, self._text(eng, gen.ids))
         except Exception as error:
             raise RuntimeError(f"Inference failed: {error}")
@@ -482,6 +502,7 @@ class NativeInferenceService:
         try:
             options = request.get("options") or {}
             num_predict = self._num_predict(options)
+            fmt = self._format(request)
             eng = await self._engine_async(request["model"])
             ids = self._prompt_ids(eng, request, request.get("prompt"))
             loop = asyncio.get_running_loop()
@@ -494,7 +515,7 @@ class NativeInferenceService:
 
             async def work():
                 try:
-                    _, gen = await self._generate(request["model"], ids, num_predict, options, on_token)
+                    _, gen = await self._generate(request["model"], ids, num_predict, options, on_token, fmt=fmt)
                     q.put_nowait(("done", gen, None))     # after every token this generation queued (same loop, FIFO)
                 except Exception as ex:          # surfaced on the consumer side
                     q.put_nowait(("err", ex, None))
@@ -535,6 +556,7 @@ class NativeInferenceService:
                 raise RuntimeError("Chat request must include messages in metadata")
             options = request.get("options") or {}
             num_predict = self._num_predict(options)
+            fmt = self._format(request)
             eng = await self._engine_async(request["model"])
             prompt = self._chat_prompt(eng, md["messages"])
             if md.get("prompt_token_ids") is not None:
@@ -543,7 +565,7 @@ class NativeInferenceService:
                 if not eng.info.has_tokenizer:
                     raise RuntimeError("model carries no tokenizer; supply metadata.prompt_token_ids")
                 ids = eng.tokenize(prompt, add_bos=True, parse_special=True)
-            eng, gen = await self._generate(request["model"], ids, num_predict, options)
+            eng, gen = await self._generate(request["model"], ids, num_predict, options, fmt=fmt)
             res = self._response(request, eng, gen, self._text(eng, gen.ids))
             res["message"] = {"role": "assistant", "content": res.pop("response")}
             return res

@@ -93,6 +93,19 @@ void read_penalty_opts(napi_env env, napi_value o, gl_sample_opts& so) {
     if (napi_get_named_property(env, o, "presencePenalty", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.presence_penalty = (float)d;
     if (napi_get_named_property(env, o, "frequencyPenalty", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.frequency_penalty = (float)d;
     if (napi_get_named_property(env, o, "minP", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.min_p = (float)d;
+    // output format: "json" (or GL_FORMAT_JSON) turns the JSON grammar mask on; absent, "" or 0 is free text; anything else
+    // reaches the library as it is and is refused there (GL_ERR_INVALID)
+    napi_valuetype vt;
+    if (napi_get_named_property(env, o, "format", &v) == napi_ok && napi_typeof(env, v, &vt) == napi_ok) {
+        if (vt == napi_string) {
+            char buf[16] = {0};
+            size_t len = 0;
+            if (napi_get_value_string_utf8(env, v, buf, sizeof buf, &len) == napi_ok)
+                so.format = len == 0 ? 0 : (std::strcmp(buf, "json") == 0 ? GL_FORMAT_JSON : -1);
+        } else if (vt == napi_number) {
+            napi_get_value_int32(env, v, &so.format);
+        }
+    }
 }
 
 // ---- generate: async work + threadsafe token callback --------------------------------------------------

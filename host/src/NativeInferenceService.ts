@@ -151,7 +151,20 @@ export class NativeInferenceService {
 		if (numPredict < 0) numPredict = nCtx > 0 ? Math.max(1, nCtx - nPrompt) : 128;
 		if (nCtx > 0 && nPrompt < nCtx) numPredict = Math.min(numPredict, nCtx - nPrompt);
 		return { numPredict, ignoreEos: !!o.ignore_eos, temperature, topK: o.top_k ?? d.top_k ?? 0, topP: o.top_p ?? d.top_p ?? 1,
-			seed: BigInt(o.seed ?? (temperature > 0 ? Math.floor(Math.random() * 2 ** 53) : 0)), ...this.penaltyOpts(o) };
+			seed: BigInt(o.seed ?? (temperature > 0 ? Math.floor(Math.random() * 2 ** 53) : 0)), ...this.penaltyOpts(o),
+			...this.formatOpts(request) };
+	}
+
+	// The output format -> the addon's format field; same mapping as gridllm_b200/service.py::_format.  metadata.format first (the
+	// gateway's Ollama routes), then options.format (its OpenAI route).  "json" turns the JSON grammar mask on; so does a JSON-schema
+	// object, whose schema is NOT enforced (the response is valid JSON of any shape).  Absent, null or "": free text.
+	private formatOpts(request: InferenceRequest): { format?: string } {
+		let f: any = request.metadata?.format;
+		if (f === undefined || f === null || f === "") f = (request.options as Record<string, any> | undefined)?.format;
+		if (f === undefined || f === null || f === "") return {};
+		if (f !== "json" && (typeof f !== "object" || Array.isArray(f))) throw new Error(`format must be "json" or a JSON schema object`);
+		if (request.options?.ignore_eos) throw new Error("format json cannot be combined with ignore_eos: a JSON document ends on a stop token");
+		return { format: "json" };
 	}
 
 	// GRIDLLM_PENALTIES=ollama: requests that leave the repetition penalty out inherit Ollama's defaults (repeat_penalty 1.1 over

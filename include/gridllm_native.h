@@ -103,8 +103,36 @@ typedef struct gl_sample_opts {
     float    presence_penalty;  /* subtracted once from every id in the window */
     float    frequency_penalty; /* subtracted once per occurrence in the window */
     float    min_p;             /* temperature > 0 only: after top-p keep the prefix of candidates with exp((l - l0) / T) >= min_p; 0 = off */
-    int32_t  reserved[1];
+    /* Output format (Ollama's `format`; 0 = off, GL_FORMAT_JSON = 1; anything else GL_ERR_INVALID).  With GL_FORMAT_JSON the
+     * bytes a sequence generates -- the concatenation of the gl_token_piece bytes of its tokens -- are held to the language
+     *   root    ::= object
+     *   value   ::= object | array | string | number | ("true" | "false" | "null") ws
+     *   object  ::= "{" ws ( string ":" ws value ( "," ws string ":" ws value )* )? "}" ws
+     *   array   ::= "[" ws ( value ( "," ws value )* )? "]" ws
+     *   string  ::= "\"" ( char | "\\" ( ["\\/bfnrt] | "u" hex hex hex hex ) )* "\"" ws
+     *   char    ::= any Unicode scalar value >= U+0020 other than " and \, as well-formed UTF-8 (a piece may end inside one)
+     *   number  ::= "-"? ( "0" | [1-9] [0-9]* ) ( "." [0-9]+ )? ( [eE] [-+]? [0-9]+ )? ws
+     *   ws      ::= "" | " " | "\n" [ \t]{0,20}
+     * with nesting depth <= 64 (root included; an opening bracket at depth 64 is masked), starting from the initial state (the
+     * prompt does not count).  Before EVERY draw (the first token after the prompt included), after the repetition penalties
+     * and before temperature / top-k / top-p / min-p / the greedy argmax, every token whose piece would take the bytes outside
+     * the language gets logit -inf; a masked token is never drawn.  Stop tokens (eos, eot when the model has one, stop_ids)
+     * are allowed only once the root object has closed, anywhere in its trailing ws, and masked everywhere else; other control
+     * tokens (empty piece) are always masked.  After the root closes only ws and stop tokens remain, so a document ends within
+     * 22 further draws (done_reason "stop"); a generation cut by num_predict is a valid prefix (done_reason "length").
+     * Reported logprobs and the logits of gl_last_logits / gl_seq_logits are those of the masked distribution.
+     * Refused: with ignore_eos (GL_ERR_INVALID); stop_ids that are not control tokens (GL_ERR_INVALID); a model without a
+     * tokenizer, or whose vocabulary lacks a single-byte token for each of \t, \n, 0x20-0x7E (and 0x80-0xBF when some piece
+     * is not whole well-formed UTF-8), or has no eos (GL_ERR_UNSUPPORTED, checked once, at the first JSON request); gl_generate
+     * on the persistent decode kernel (GL_MEGA=1, GL_ERR_UNSUPPORTED).  JSON schemas are not enforced here: a host maps a
+     * schema to GL_FORMAT_JSON and gets valid JSON of any shape. */
+    union {
+        int32_t  format;
+        int32_t  reserved[1];
+    };
 } gl_sample_opts;
+
+#define GL_FORMAT_JSON 1
 
 typedef struct gl_gen_stats {
     int32_t prompt_eval_count;     /* InferenceResponse.prompt_eval_count (client/src/types/index.ts:61) */
@@ -162,8 +190,8 @@ int  gl_embed(gl_engine* e, const int32_t* ids, const int32_t* seq_offsets, int3
  *                 the token drawn was a stop token (not part of the output).  Finished sequences stay open, holding
  *                 their pages, until gl_seq_close.  *n = entries written (<= cap).
  *   gl_seq_close  return the slot and its pages.
- *   gl_seq_logits logits [n_vocab] the sequence's LAST token was drawn from, penalties applied (parity tests; valid until the
- *                 next step).
+ *   gl_seq_logits logits [n_vocab] the sequence's LAST token was drawn from, penalties and the JSON mask applied (parity
+ *                 tests; valid until the next step).
  * Sequences join and leave between steps; a sequence's tokens do not depend on who shares its batch. */
 int  gl_seq_open(gl_engine* e, const int32_t* prompt, int32_t n_prompt, const gl_sample_opts* opts, int32_t* slot);
 /* Several prompts in one call: they share one packed prompt pass (block-diagonal causal attention, every weight matrix read
@@ -195,8 +223,8 @@ int  gl_batch_counters(gl_engine* e, uint64_t out[8], int32_t reset);
 int  gl_time_batch_step(gl_engine* e, int32_t batch, int32_t ctx_len, int32_t iters, float* ms_per_step, int32_t* launches_per_step,
                         uint64_t* weight_bytes);
 
-/* logits of generation step i of the last gl_generate that ran with want_logits=1 (after the repetition penalties, if the
- * request had any: the logits the token was drawn from) */
+/* logits of generation step i of the last gl_generate that ran with want_logits=1 (after the repetition penalties and the
+ * JSON mask, if the request had them: the logits the token was drawn from) */
 int  gl_last_logits(gl_engine* e, int32_t step, float* out, int32_t n_vocab);
 
 /* the sampler alone on caller-supplied logits [n_vocab]: the token gl_generate would emit as output number out_index
@@ -211,6 +239,13 @@ int  gl_sample_logits(gl_engine* e, const float* logits, int32_t n_vocab, const 
  * like gl_kv_reset(). */
 int  gl_penalize_logits(gl_engine* e, float* logits, int32_t n_vocab, const gl_sample_opts* opts, const int32_t* history,
                         int32_t n_history);
+/* the JSON grammar mask alone, in place on caller-supplied logits [n_vocab]: the state the device automaton reaches from the
+ * initial state through generated[0..n_generated) (the output so far), then the mask kernel (opts->format; format 0 leaves the
+ * logits as they are; the stop tokens are eos / eot / opts->stop_ids).  GL_ERR_INVALID when generated is not a prefix the mask
+ * allows.  Parity tests against tests/json_oracle.py; hosts may probe for this symbol to learn that format is honoured.
+ * Rewinds the sequence like gl_kv_reset(). */
+int  gl_constrain_logits(gl_engine* e, float* logits, int32_t n_vocab, const gl_sample_opts* opts, const int32_t* generated,
+                         int32_t n_generated);
 
 /* ---- kernel-level entry points (parity tests and roofline measurement) ------------------ */
 /* y[rows] = W[rows x cols] (GGUF-layout blocks of ggml_type, host memory) * x[cols].
