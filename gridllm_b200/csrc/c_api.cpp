@@ -51,6 +51,11 @@ const char* check_penalties(const gl_sample_opts& so) {
 // format took the place of the last reserved word (an anonymous union keeps `reserved` addressable): a zeroed word is "off"
 static_assert(offsetof(gl_sample_opts, format) == 64, "format sits where reserved[0] was");
 
+// prefix_cache took the place of gl_engine_opts.reserved[0]: the size and the older offsets are unchanged, a zeroed word is "off"
+static_assert(sizeof(gl_engine_opts) == 64, "gl_engine_opts size is part of the ABI");
+static_assert(offsetof(gl_engine_opts, batch_weights) == 28 && offsetof(gl_engine_opts, prefix_cache) == 32 &&
+                  offsetof(gl_engine_opts, reserved) == 36, "prefix_cache sits where reserved[0] was");
+
 // the format field of a generating request; nullptr when valid
 const char* check_format(const gl_sample_opts& so) {
     if (so.format != 0 && so.format != GL_FORMAT_JSON) return "format must be 0 (off) or GL_FORMAT_JSON";

@@ -12,6 +12,7 @@
 
 #include "common.cuh"
 #include "json_fsm.h"
+#include "prefix_reuse.h"
 #include "rowdot.h"
 
 namespace gl {
@@ -188,6 +189,7 @@ Status Engine::load(const std::string& path, int device, const gl_engine_opts* o
     prefill_tc5_ = env_int("GL_PREFILL_TC5", 1) != 0;
     prefill_flash_ = env_int("GL_PREFILL_FLASH", 1) != 0;
     prefill_fuse_rope_ = env_int("GL_PREFILL_FUSE_ROPE", 1) != 0;
+    prefix_cache_ = opts && opts->prefix_cache != 0;
 
     std::string err = gguf_.open(path);
     if (!err.empty()) return fail(err.find("cannot open") == 0 ? GL_ERR_IO : GL_ERR_FORMAT, err);
@@ -412,6 +414,7 @@ const DevMatrix* Engine::find_matrix(const std::string& name) const {
 Status Engine::kv_reset() {
     for (int p : seq_pages_) free_pages_.push_back(p);
     seq_pages_.clear();
+    cached_ids_.clear();
     host_pos_ = 0;
     return set_state(0, 0, 0, 0, nullptr);
 }
@@ -817,7 +820,14 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
     ST(json_admit(so, true));
     for (int i = 0; i < n_prompt; ++i)
         if (prompt[i] < 0 || prompt[i] >= n_vocab_) return fail(GL_ERR_INVALID, "prompt token id out of range");
-    ST(kv_reset());
+    // prefix reuse: keep the pages of the positions the previous request left final and that this prompt repeats
+    const int reuse = (prefix_cache_ && !use_mega_) ? prefix_reuse(prompt, n_prompt, cached_ids_.data(), (int)cached_ids_.size(), prefill_min_) : 0;
+    if (reuse > 0) {
+        cached_ids_.clear();                         // rebuilt below once this request's K / V are final
+        host_pos_ = reuse;
+    } else {
+        ST(kv_reset());
+    }
     ST(ensure_pages(n_prompt + n_pred));
     if (so.want_logits) {
         if (keep_cap_ < n_pred) {
@@ -832,23 +842,24 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
                         if (g) { cudaGraphExecDestroy(g); g = nullptr; }      // captured with the old logits buffer
         }
     }
+    // the whole prompt is the penalty history, whatever part of it is reused
     CU(cudaMemcpyAsync(prompt_ids_, prompt, (size_t)n_prompt * 4, cudaMemcpyHostToDevice, stream_));
-    const bool batched = can_batch_prefill(n_prompt);
+    const bool batched = can_batch_prefill(reuse, n_prompt - reuse);
     int prefill_launches = 0;
     const int mega0 = mega_launches_;
     if (batched) {
-        // whole prompt through the tensor-core path; the sampler then moves pos from T-1 to T
+        // prompt positions [reuse, n_prompt) through the tensor-core path; the sampler then moves pos from T-1 to T
         ST(set_state(n_prompt - 1, prompt[n_prompt - 1], n_prompt, 0, &so));
         CU(cudaEventRecord(ev_[0], stream_));
-        ST(prefill_batched(n_prompt, &prefill_launches));
+        ST(prefill_batched(reuse, n_prompt - reuse, &prefill_launches));
         CU(cudaEventRecord(ev_[1], stream_));
     } else {
-        // sequential prefill: n_prompt-1 positions without a head, then the last prompt token produces token 0
-        ST(set_state(0, prompt[0], n_prompt, 0, &so));
+        // sequential prefill: positions reuse .. n_prompt-2 without a head, then the last prompt token produces token 0
+        ST(set_state(reuse, prompt[reuse], n_prompt, 0, &so));
         CU(cudaEventRecord(ev_[0], stream_));
-        ST(run_steps(n_prompt - 1, 0, false));
+        ST(run_steps(n_prompt - 1 - reuse, 0, false));
         CU(cudaEventRecord(ev_[1], stream_));
-        prefill_launches = use_mega_ ? 0 : (n_prompt - 1) * launches_nohead_;
+        prefill_launches = use_mega_ ? 0 : (n_prompt - 1 - reuse) * launches_nohead_;
     }
     bool first_head_only = batched;
 
@@ -890,11 +901,19 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
     CU(cudaEventSynchronize(ev_[2]));
     if (cancelled) done_reason = 2;
     host_pos_ = n_prompt + produced;
+    if (prefix_cache_ && !use_mega_) {
+        // K / V are final for the prompt and for every generated id the device has FED: a step feeds output i - 1 while it draws
+        // output i, so hs.out_idx draws fed hs.out_idx - 1 of them.  The last draw (and a stop token) was never fed; steps the
+        // device ran past what the host reported (a cancel mid-chunk, a stop) fed ids the host did not record and stay out.
+        const int fed = std::max(0, std::min(produced, hs.out_idx - 1));
+        cached_ids_.assign(prompt, prompt + n_prompt);
+        cached_ids_.insert(cached_ids_.end(), ids.begin(), ids.begin() + fed);
+    }
     if (stats) {
         float ms_p = 0.f, ms_d = 0.f;
         cudaEventElapsedTime(&ms_p, ev_[0], ev_[1]);
         cudaEventElapsedTime(&ms_d, ev_[1], ev_[2]);
-        stats->prompt_eval_count = n_prompt;
+        stats->prompt_eval_count = n_prompt - reuse;
         stats->eval_count = produced;
         stats->prompt_eval_duration_ns = (int64_t)(ms_p * 1e6);
         stats->eval_duration_ns = (int64_t)(ms_d * 1e6);
@@ -1105,6 +1124,7 @@ Status Engine::constrain_logits(float* logits, int n_vocab, const gl_sample_opts
 Status Engine::decode_step(int token, float* logits, int* argmax, float* logprob) {
     CU(cudaSetDevice(device_));
     if (token < 0 || token >= n_vocab_) return fail(GL_ERR_INVALID, "token id out of range");
+    cached_ids_.clear();                              // the pages and the step state are now this call's: no prefix reuse
     ST(ensure_pages(host_pos_ + 1));
     gl_sample_opts so{};
     so.ignore_eos = 1;
@@ -1127,18 +1147,20 @@ Status Engine::prefill(const int32_t* ids, int n, float* last_logits) {
     if (n <= 0) return fail(GL_ERR_INVALID, "empty prefill");
     for (int i = 0; i < n; ++i)
         if (ids[i] < 0 || ids[i] >= n_vocab_) return fail(GL_ERR_INVALID, "token id out of range");
+    cached_ids_.clear();                              // the pages and the step state are now this call's: no prefix reuse
     ST(ensure_pages(host_pos_ + n));
     gl_sample_opts so{};
     so.ignore_eos = 1;
-    if (can_batch_prefill(n)) {
+    // both paths read the tokens from prompt_ids_ indexed by absolute position
+    CU(cudaMemcpyAsync(prompt_ids_ + host_pos_, ids, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
+    if (can_batch_prefill(host_pos_, n)) {
+        // positions [host_pos_, host_pos_ + n) on the tensor cores, attending to everything before them through the pages
         int dummy = 0;
-        CU(cudaMemcpyAsync(prompt_ids_, ids, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
-        ST(set_state(n - 1, ids[n - 1], n, 0, &so));
-        ST(prefill_batched(n, &dummy));
+        ST(set_state(host_pos_ + n - 1, ids[n - 1], host_pos_ + n, 0, &so));
+        ST(prefill_batched(host_pos_, n, &dummy));
         ST(enqueue_head(stream_, false, &dummy));
     } else {
-        // sequential prefill: tokens are fed from prompt_ids_ indexed by absolute position
-        CU(cudaMemcpyAsync(prompt_ids_ + host_pos_, ids, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
+        // sequential prefill
         ST(set_state(host_pos_, ids[0], host_pos_ + n, 0, &so));
         ST(run_steps(n - 1, 1, false));
     }
@@ -1209,10 +1231,23 @@ Status Engine::embed(const int32_t* ids, const int32_t* offs, int n_seq, float* 
                 gl_sample_opts so{};
                 so.ignore_eos = 1;
                 ST(set_state(0, ids[offs[sidx]], n, 0, &so));
-                if (!can_batch_prefill(n)) return fail(GL_ERR_CONTEXT, "sequence too long for the batched prompt pass");
-                ST(prefill_batched(n, &launches));
-                CU(pool_embedding_launch(pf_x_, n, n_embd_, output_norm_, eps_, emb_rstd_, emb_pooled_, emb_out_ + (size_t)sidx * n_embd_, stream_));
-                launches += 3;
+                if (!can_batch_prefill(0, n)) return fail(GL_ERR_UNSUPPORTED, "a sequence longer than one prompt pass needs the fused prompt attention");
+                if (n <= PF_CHUNK) {
+                    ST(prefill_batched(0, n, &launches));
+                    CU(pool_embedding_launch(pf_x_, n, n_embd_, output_norm_, eps_, emb_rstd_, emb_pooled_, emb_out_ + (size_t)sidx * n_embd_, stream_));
+                    launches += 3;
+                } else {
+                    // passes of PF_CHUNK rows (each attends to the earlier ones through the pages); the pooling sums the
+                    // normalised columns of every pass, then scales and L2-normalises once
+                    for (int c0 = 0; c0 < n; c0 += PF_CHUNK) {
+                        const int len = std::min(PF_CHUNK, n - c0);
+                        ST(prefill_chunk(c0, len, &launches));
+                        CU(pool_embedding_sum_launch(pf_x_, len, n_embd_, eps_, emb_rstd_, emb_pooled_, c0 > 0, stream_));
+                        launches += 2;
+                    }
+                    CU(pool_embedding_finish_launch(emb_pooled_, n, n_embd_, output_norm_, emb_out_ + (size_t)sidx * n_embd_, stream_));
+                    launches += 2;
+                }
                 ++sidx;
                 continue;
             }

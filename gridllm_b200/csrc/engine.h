@@ -103,7 +103,10 @@ private:
     Status build_mega();
     Status launch_mega(int n_steps, bool with_head, bool keep_logits);
     Status ensure_prefill_scratch(int t_pad);
-    Status prefill_batched(int n, int* n_launch);     // tokens already in prompt_ids_[0..n)
+    // positions [pos0, pos0 + n) of the single sequence, tokens already in prompt_ids_[pos0 .. pos0 + n), in passes of <= PF_CHUNK rows
+    Status prefill_batched(int pos0, int n, int* n_launch);
+    Status prefill_chunk(int pos0, int n, int* n_launch);
+    static constexpr int PF_CHUNK = 4096;             // rows of one prompt pass (the prefill scratch never grows past it)
     // embeddings: several sequences in ONE prompt pass (block-diagonal causal attention); seq s = rows [starts[s], starts[s] + lens[s])
     // tables: per sequence, the device page table its K / V rows are cached through (null: nothing is cached -- embeddings)
     Status prefill_packed(const std::vector<int>& starts, const std::vector<int>& lens, int t_rows, int* n_launch,
@@ -112,7 +115,15 @@ private:
     int* pk_ids_ = nullptr;                           // [EMB_PACK_TOKENS] token ids of a pack (pad rows: token 0)
     float *emb_out_ = nullptr, *emb_rstd_ = nullptr, *emb_pooled_ = nullptr;
     int emb_out_cap_ = 0;
-    bool can_batch_prefill(int n) const { return have_w16_ && prefill_mode_ != 1 && host_pos_ == 0 && n >= prefill_min_ && n <= 4096; }
+    // n tokens from position pos0 through the tensor-core prompt pass; a pass that does not start at 0 (a later chunk of a long
+    // prompt included) needs the fused prompt attention, so under GL_PREFILL_FLASH=0 such a prompt stays sequential
+    bool can_batch_prefill(int pos0, int n) const {
+        return have_w16_ && prefill_mode_ != 1 && n >= prefill_min_ && (prefill_flash_ || (pos0 == 0 && n <= PF_CHUNK));
+    }
+    // gl_generate's prefix reuse (gl_engine_opts.prefix_cache): ids at positions [0, cached_ids_.size()) whose K / V in the
+    // single-sequence pages are final; cleared by everything else that writes those pages or the step state
+    bool prefix_cache_ = false;
+    std::vector<int32_t> cached_ids_;
     const DevMatrix* find_matrix(const std::string& name) const;
 
     // model

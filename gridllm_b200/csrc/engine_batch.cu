@@ -283,9 +283,9 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
         cudaError_t ce = cudaMemcpyAsync(prompt_ids_, prompt, (size_t)n_prompt * 4, cudaMemcpyHostToDevice, stream_);
         if (ce == cudaSuccess) ce = cudaEventRecord(ev_[2], stream_);
         if (ce != cudaSuccess) { rs = failb(GL_ERR_CUDA, cudaGetErrorString(ce)); break; }
-        if (can_batch_prefill(n_prompt)) {
+        if (can_batch_prefill(0, n_prompt)) {      // any length: passes of PF_CHUNK rows, the later ones over the slot's pages
             rs = set_state(n_prompt - 1, prompt[n_prompt - 1], n_prompt, 0, &so);
-            if (rs.ok()) rs = prefill_batched(n_prompt, &dummy);
+            if (rs.ok()) rs = prefill_batched(0, n_prompt, &dummy);
             if (rs.ok()) rs = enqueue_head(stream_, false, &dummy);
         } else {      // short prompts: plain launches of the decode step (the captured graphs hold the engine's own pointers)
             rs = set_state(0, prompt[0], n_prompt, 0, &so);

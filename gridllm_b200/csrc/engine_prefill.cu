@@ -86,9 +86,31 @@ Status Engine::ensure_prefill_scratch(int t_pad) {
     return {};
 }
 
-Status Engine::prefill_batched(int n, int* n_launch) {
+// Positions [pos0, pos0 + n) of the single sequence, in passes of at most PF_CHUNK rows: each pass is one segment
+// {start 0, len, pos0 of the pass, page_table_}, so its K / V rows land in the pages before its attention reads them, and a
+// pass that does not start at 0 attends to everything before it through the pages (the PAGED prompt attention).  A prompt of
+// at most PF_CHUNK tokens from position 0 is the one pass it always was.
+Status Engine::prefill_batched(int pos0, int n, int* n_launch) {
+    int nl = 0;
+    for (int c0 = 0; c0 < n; c0 += PF_CHUNK) {
+        const int len = std::min(PF_CHUNK, n - c0);
+        int nc = 0;
+        ST(prefill_chunk(pos0 + c0, len, &nc));
+        nl += nc;
+    }
+    // hidden state of the last prompt token -> the decode path's x buffer (lm_head / sampler follow)
+    const int last = (n - 1) % PF_CHUNK;
+    CU(cudaMemcpyAsync(x_, pf_x_ + (size_t)last * n_embd_, (size_t)n_embd_ * 4, cudaMemcpyDeviceToDevice, stream_));
+    if (n_launch) *n_launch += nl;
+    last_prefill_launches_ = nl;
+    return {};
+}
+
+// One pass of prefill_batched: positions [pos0, pos0 + n), n <= PF_CHUNK; hidden states end up in pf_x_ rows 0 .. n - 1
+Status Engine::prefill_chunk(int pos0, int n, int* n_launch) {
     const int T = n, TP = (n + 127) / 128 * 128;
     const int qd = n_head_ * hd_, kvd = n_kv_ * hd_, ldq = qd + 2 * kvd, grp = n_head_ / n_kv_;
+    if (pos0 > 0 && !prefill_flash_) return failp(GL_ERR_UNSUPPORTED, "a prompt pass from a non-zero position needs the fused prompt attention");
     ST(ensure_prefill_scratch(TP));
     const int tp = pf_cap_;          // leading dimension of the [T_pad]-shaped scratch
     cudaStream_t s = stream_;
@@ -99,10 +121,10 @@ Status Engine::prefill_batched(int n, int* n_launch) {
         if (prefill_tc5_ && gemm_tc5_supported(g)) return gemm_tc5_launch(g, tp, bf, s);
         return gemm_tn_launch(g, bf, s);
     };
-    CU(embed_rows_launch(tok_embd_.w, tok_embd_.type, n_embd_, tok_embd_.row_stride, prompt_ids_, T, pf_x_, s)); ++nl;
+    CU(embed_rows_launch(tok_embd_.w, tok_embd_.type, n_embd_, tok_embd_.row_stride, prompt_ids_ + pos0, T, pf_x_, s)); ++nl;
     const float scale = 1.0f / std::sqrt((float)hd_);
     PrefillSegs segs{};
-    segs.n = 1; segs.start[0] = 0; segs.len[0] = T; segs.table[0] = page_table_;
+    segs.n = 1; segs.start[0] = 0; segs.len[0] = T; segs.table[0] = page_table_; segs.pos0[0] = pos0;
     for (int il = 0; il < n_layer_; ++il) {
         const LayerWeights& L = layers_[il];
         __half* kc = kcache_ + (size_t)il * kv_layer_elems_;
@@ -126,7 +148,7 @@ Status Engine::prefill_batched(int n, int* n_launch) {
         if (prefill_flash_) {
             // (RoPE + split + cache append, then) ONE fused attention launch (prefill_attn.cu): scores stay on the SM
             if (!roped) { CU(rope_split_segs_launch(pf_qkv_, TP, n_head_, n_kv_, hd_, rope_cos_, rope_sin_, pf_q_, pf_k_, pf_vt_, kc, vc, tp, segs, s)); ++nl; }
-            CU(flash_prefill_launch(pf_q_, pf_k_, pf_vt_, (__half*)pf_attn_, segs, n_head_, n_kv_, hd_, tp, scale, s));
+            CU(flash_prefill_launch(pf_q_, pf_k_, pf_vt_, (__half*)pf_attn_, segs, n_head_, n_kv_, hd_, tp, scale, kc, vc, s));
             ++nl;
         } else {
             CU(rope_split_launch(pf_qkv_, T, tp, 0, n_head_, n_kv_, hd_, rope_cos_, rope_sin_, pf_q_, pf_k_, pf_vt_, kc, vc, page_table_, tp, s)); ++nl;
@@ -166,10 +188,7 @@ Status Engine::prefill_batched(int n, int* n_launch) {
             CU(linear(g)); ++nl;
         }
     }
-    // hidden state of the last prompt token -> the decode path's x buffer (lm_head / sampler follow)
-    CU(cudaMemcpyAsync(x_, pf_x_ + (size_t)(T - 1) * n_embd_, (size_t)n_embd_ * 4, cudaMemcpyDeviceToDevice, s));
     if (n_launch) *n_launch += nl;
-    last_prefill_launches_ = nl;
     return {};
 }
 
@@ -237,7 +256,7 @@ Status Engine::prefill_packed(const std::vector<int>& starts, const std::vector<
                     CU(rope_split_segs_launch(pf_qkv_ + (size_t)row_lo * ldq, row_hi - row_lo, n_head_, n_kv_, hd_, rope_cos_, rope_sin_, pf_q_ + (size_t)row_lo * qd,
                                               pf_k_ + (size_t)row_lo * kvd, pf_vt_ + row_lo, kc, vc, tp, rs, s)); ++nl;
                 }
-                CU(flash_prefill_launch(pf_q_, pf_k_, pf_vt_, (__half*)pf_attn_, segs, n_head_, n_kv_, hd_, tp, scale, s));
+                CU(flash_prefill_launch(pf_q_, pf_k_, pf_vt_, (__half*)pf_attn_, segs, n_head_, n_kv_, hd_, tp, scale, kc, vc, s));
                 ++nl;
             }
         } else

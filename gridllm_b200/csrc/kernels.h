@@ -192,6 +192,11 @@ cudaError_t add_launch(const float* a, const float* b, int n, float* out, cudaSt
 // generateEmbedding: out[n] = L2-normalised mean over rows of RMSNorm(h_t) * norm_w;  scratch: rstd [rows], pooled [n]
 cudaError_t pool_embedding_launch(const float* h, int rows, int n, const float* norm_w, float eps, float* rstd_scratch, float* pooled_scratch,
                                   float* out, cudaStream_t s);
+// the same pooling over a sequence that arrives in several prompt passes: each pass adds the column sums of its rows' RMSNorm(h_t)
+// (without norm_w) to sum [n] (accumulate = 0: the first pass overwrites it); the finish scales by norm_w / total_rows in place
+// and L2-normalises into out
+cudaError_t pool_embedding_sum_launch(const float* h, int rows, int n, float eps, float* rstd_scratch, float* sum, bool accumulate, cudaStream_t s);
+cudaError_t pool_embedding_finish_launch(float* sum, int total_rows, int n, const float* norm_w, float* out, cudaStream_t s);
 cudaError_t l2_flush_launch(float* buf, size_t n, cudaStream_t s);
 
 }  // namespace gl

@@ -250,6 +250,18 @@ __global__ void __launch_bounds__(256) pool_cols_kernel(const float* __restrict_
     for (int t = 0; t < rows; ++t) acc += h[(size_t)t * n + d] * rstd[t];
     pooled[d] = acc * w[d] / (float)rows;
 }
+__global__ void __launch_bounds__(256) pool_sum_kernel(const float* __restrict__ h, const float* __restrict__ rstd, int rows, int n,
+                                                       int accumulate, float* __restrict__ sum) {
+    const int d = blockIdx.x * 256 + threadIdx.x;
+    if (d >= n) return;
+    float acc = 0.f;
+    for (int t = 0; t < rows; ++t) acc += h[(size_t)t * n + d] * rstd[t];
+    sum[d] = accumulate ? sum[d] + acc : acc;
+}
+__global__ void __launch_bounds__(256) pool_scale_kernel(float* __restrict__ sum, const float* __restrict__ w, int rows, int n) {
+    const int d = blockIdx.x * 256 + threadIdx.x;
+    if (d < n) sum[d] = sum[d] * w[d] / (float)rows;
+}
 __global__ void __launch_bounds__(1024) pool_normalize_kernel(const float* __restrict__ pooled, int n, float* __restrict__ out) {
     __shared__ float red[32];
     float ss = 0.f;
@@ -313,6 +325,16 @@ cudaError_t pool_embedding_launch(const float* h, int rows, int n, const float* 
     pool_rstd_kernel<<<rows, 256, 0, s>>>(h, rows, n, eps, rstd_scratch);
     pool_cols_kernel<<<(n + 255) / 256, 256, 0, s>>>(h, rstd_scratch, norm_w, rows, n, pooled_scratch);
     pool_normalize_kernel<<<1, 1024, 0, s>>>(pooled_scratch, n, out);
+    return cudaGetLastError();
+}
+cudaError_t pool_embedding_sum_launch(const float* h, int rows, int n, float eps, float* rstd_scratch, float* sum, bool accumulate, cudaStream_t s) {
+    pool_rstd_kernel<<<rows, 256, 0, s>>>(h, rows, n, eps, rstd_scratch);
+    pool_sum_kernel<<<(n + 255) / 256, 256, 0, s>>>(h, rstd_scratch, rows, n, accumulate ? 1 : 0, sum);
+    return cudaGetLastError();
+}
+cudaError_t pool_embedding_finish_launch(float* sum, int total_rows, int n, const float* norm_w, float* out, cudaStream_t s) {
+    pool_scale_kernel<<<(n + 255) / 256, 256, 0, s>>>(sum, norm_w, total_rows, n);
+    pool_normalize_kernel<<<1, 1024, 0, s>>>(sum, n, out);
     return cudaGetLastError();
 }
 

@@ -15,13 +15,15 @@ enum GemmEpilogue : int {
 };
 
 // The sequences of one prompt pass: sequence i owns rows [start[i], start[i] + len[i]) of the packed activation matrix (starts at
-// 128-row boundaries); table[i] = its KV page table on the device (null: nothing is cached).
+// 128-row boundaries); table[i] = its KV page table on the device (null: nothing is cached).  pos0[i] = the absolute position
+// of its first row (0 for a whole prompt; > 0 for a chunk that continues a sequence whose earlier positions are in its pages).
 constexpr int PF_MAX_SEGS = 32;
 struct PrefillSegs {
     int n;
     int start[PF_MAX_SEGS];
     int len[PF_MAX_SEGS];
     const int* table[PF_MAX_SEGS];
+    int pos0[PF_MAX_SEGS];
 };
 // what GEMM_EPI_ROPE_SPLIT writes instead of C (the arguments of rope_split_segs_launch, which it replaces)
 struct RopeSplitArgs {
@@ -69,9 +71,11 @@ cudaError_t rope_split_launch(const float* qkv, int t_rows, int t_pad, int pos0,
 // ---- fused prompt attention (prefill_attn.cu) --------------------------------------------------------------------
 cudaError_t flash_prefill_configure();
 bool flash_prefill_supported(int hd);
-// out[rows][n_head * hd] = causal softmax(q k^T * scale) v per sequence and head; q / k rows, vt = V^T [n_kv * hd][vt_ld]
+// out[rows][n_head * hd] = causal softmax(q k^T * scale) v per sequence and head; q / k rows, vt = V^T [n_kv * hd][vt_ld].
+// When some segment has pos0 > 0, its query rows attend to keys 0 .. pos0 + len - 1 read from this layer's fp16 pages
+// (k_cache / v_cache through segs.table; the segment's own rows must already be appended) and k / vt are not read.
 cudaError_t flash_prefill_launch(const __half* q, const __half* k, const __half* vt, __half* out, const PrefillSegs& segs, int n_head, int n_kv,
-                                 int hd, int vt_ld, float scale, cudaStream_t s);
+                                 int hd, int vt_ld, float scale, const __half* k_cache, const __half* v_cache, cudaStream_t s);
 // rope_split for every sequence of a pack in one launch (rows_pad = rows of the pack, padding rows are zeroed)
 cudaError_t rope_split_segs_launch(const float* qkv, int rows_pad, int n_head, int n_kv, int hd, const float* cos_t, const float* sin_t, __half* qo,
                                    __half* ko, __half* vt, __half* k_cache, __half* v_cache, int vt_ld, const PrefillSegs& segs, cudaStream_t s);

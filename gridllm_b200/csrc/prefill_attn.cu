@@ -30,7 +30,9 @@ struct FlashParams {
     const __half* k;     // [rows][kvd]
     const __half* vt;    // [kvd][vt_ld]
     __half* out;         // [rows][qd]
-    int qd, kvd, vt_ld, grp;
+    const __half* k_cache;   // PAGED: this layer's pages [page][n_kv][16][hd]
+    const __half* v_cache;
+    int qd, kvd, vt_ld, grp, n_kv;
     float scale_log2;    // 1/sqrt(hd) * log2(e)
     PrefillSegs segs;
 };
@@ -43,6 +45,9 @@ __device__ __forceinline__ void fa_commit() { asm volatile("cp.async.commit_grou
 template <int N> __device__ __forceinline__ void fa_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void fa_ldsm4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
+}
+__device__ __forceinline__ void fa_ldsm4t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
 }
 __device__ __forceinline__ void fa_mma(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
     asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
@@ -57,7 +62,15 @@ __device__ __forceinline__ float fa_exp2(float x) {
 // tile of 64-column rows (128 B): 16-byte chunk c of row r lives at chunk c ^ (r & 7)
 __device__ __forceinline__ uint32_t fa_swz(int row, int chunk) { return (uint32_t)(row * 128 + ((chunk ^ (row & 7)) << 4)); }
 
-template <int HD>
+// PAGED = false: keys / values of the pass's own rows, from the scratch K rows and V^T columns (a segment that starts at
+// position 0).  PAGED = true: query rows at absolute positions pos0 .. pos0 + len - 1 attend to keys 0 .. pos0 + len - 1, read
+// from the layer's fp16 pages through the segment's page table (the QKV epilogue of this layer appended the segment's own rows
+// one launch earlier).  KV tile kt is absolute positions [64 kt, 64 kt + 64) = four pages; one page of one KV head is a
+// contiguous [16][HD] block.  V arrives row-major ([kv][hd]) and is staged like K; its P V operand is loaded with
+// ldmatrix.trans, which hands every lane the same values in the same registers as the plain ldmatrix of V^T does, so both
+// variants feed the MMAs identical operands and visit the same absolute KV tiles in the same order: a prompt prefilled in
+// pieces gives the bits of one pass.
+template <int HD, bool PAGED>
 __global__ void __launch_bounds__(FA_THREADS, 2) flash_prefill_kernel(const __grid_constant__ FlashParams p) {
     // a [rows][HD] tile is HD / 64 sub-tiles of 64 columns (one 128-byte swizzle row each)
     constexpr int Q_BYTES = FA_BM * HD * 2;
@@ -68,31 +81,53 @@ __global__ void __launch_bounds__(FA_THREADS, 2) flash_prefill_kernel(const __gr
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int seq = blockIdx.z, h = blockIdx.x;
     const int len = p.segs.len[seq], r0 = p.segs.start[seq];
+    const int pos0 = PAGED ? p.segs.pos0[seq] : 0;    // absolute position of the segment's first row
     const int n_qt = (len + FA_BM - 1) / FA_BM;
     if ((int)blockIdx.y >= n_qt) return;
     const int qt = n_qt - 1 - (int)blockIdx.y;        // the longest tiles of a sequence first
     const int m0 = qt * FA_BM;
     const int kvh = h / p.grp;
-    const int n_kt = min((len + FA_BN - 1) / FA_BN, (m0 + FA_BM) / FA_BN);
+    const int kv_len = pos0 + len;                    // keys 0 .. kv_len - 1
+    const int n_kt = PAGED ? min((kv_len + FA_BN - 1) / FA_BN, (pos0 + m0 + FA_BM - 1) / FA_BN + 1)
+                           : min((len + FA_BN - 1) / FA_BN, (m0 + FA_BM) / FA_BN);
     const uint32_t sq = smem_u32(smem), sk0 = sq + Q_BYTES;
 
     const __half* qg = p.q + (size_t)(r0 + m0) * p.qd + (size_t)h * HD;
     const __half* kg = p.k + (size_t)r0 * p.kvd + (size_t)kvh * HD;
     const __half* vg = p.vt + (size_t)kvh * HD * p.vt_ld + r0;
+    const int* table = PAGED ? p.segs.table[seq] : nullptr;
+    const size_t page_elems = (size_t)p.n_kv * KV_PAGE_TOKENS * HD;
+    const __half* kcg = PAGED ? p.k_cache + (size_t)kvh * KV_PAGE_TOKENS * HD : nullptr;
+    const __half* vcg = PAGED ? p.v_cache + (size_t)kvh * KV_PAGE_TOKENS * HD : nullptr;
 
     auto load_kv = [&](int stage, int kt) {
         const int kv0 = kt * FA_BN;
         const uint32_t sk = sk0 + stage * STAGE_BYTES, sv = sk + K_BYTES;
+        if constexpr (PAGED) {
+            // K and V rows alike: [64 kv][HD] tiles; positions past the sequence are zero-filled (their scores are masked, but
+            // P V multiplies P = 0 by V, and an unused page slot may hold anything) and their page entries are never read
 #pragma unroll
-        for (int i = 0; i < (FA_BN * HD / 8) / FA_THREADS; ++i) {
-            const int idx = tid + i * FA_THREADS, r = idx / (HD / 8), c = idx % (HD / 8);
-            const bool ok = kv0 + r < len;
-            fa_cp16(sk + (c >> 3) * (FA_BN * 128) + fa_swz(r, c & 7), kg + (size_t)(ok ? kv0 + r : 0) * p.kvd + c * 8, ok);
-        }
+            for (int i = 0; i < (FA_BN * HD / 8) / FA_THREADS; ++i) {
+                const int idx = tid + i * FA_THREADS, r = idx / (HD / 8), c = idx % (HD / 8);
+                const int pos = kv0 + r;
+                const bool ok = pos < kv_len;
+                const size_t off = ok ? (size_t)__ldg(table + pos / KV_PAGE_TOKENS) * page_elems + (size_t)(pos % KV_PAGE_TOKENS) * HD + c * 8 : 0;
+                const uint32_t so = (c >> 3) * (FA_BN * 128) + fa_swz(r, c & 7);
+                fa_cp16(sk + so, kcg + off, ok);
+                fa_cp16(sv + so, vcg + off, ok);
+            }
+        } else {
 #pragma unroll
-        for (int i = 0; i < (HD * FA_BN / 8) / FA_THREADS; ++i) {
-            const int idx = tid + i * FA_THREADS, r = idx >> 3, c = idx & 7;      // r = head dim, c = chunk of 8 kv columns
-            fa_cp16(sv + fa_swz(r, c), vg + (size_t)r * p.vt_ld + kv0 + c * 8, true);
+            for (int i = 0; i < (FA_BN * HD / 8) / FA_THREADS; ++i) {
+                const int idx = tid + i * FA_THREADS, r = idx / (HD / 8), c = idx % (HD / 8);
+                const bool ok = kv0 + r < len;
+                fa_cp16(sk + (c >> 3) * (FA_BN * 128) + fa_swz(r, c & 7), kg + (size_t)(ok ? kv0 + r : 0) * p.kvd + c * 8, ok);
+            }
+#pragma unroll
+            for (int i = 0; i < (HD * FA_BN / 8) / FA_THREADS; ++i) {
+                const int idx = tid + i * FA_THREADS, r = idx >> 3, c = idx & 7;      // r = head dim, c = chunk of 8 kv columns
+                fa_cp16(sv + fa_swz(r, c), vg + (size_t)r * p.vt_ld + kv0 + c * 8, true);
+            }
         }
     };
 
@@ -107,11 +142,14 @@ __global__ void __launch_bounds__(FA_THREADS, 2) flash_prefill_kernel(const __gr
     fa_commit();
 
     const int g = lane >> 2, t4 = lane & 3;
-    const int wrow0 = m0 + warp * 32;                 // first query row of this warp (relative to the sequence)
+    const int wq0 = m0 + warp * 32;                   // first query row of this warp (relative to the segment)
+    const int wrow0 = pos0 + wq0;                     // ... its absolute position (what the mask compares with kv columns)
     // lane-dependent part of the ldmatrix addresses (k-step 0).  A operand (Q): row = lane & 15, chunk bit = lane >> 4;
-    // B operands (K, V^T): row = (lane & 7) + 8 (lane >> 4), chunk bit = (lane >> 3) & 1.
+    // B operands (K, V^T): row = (lane & 7) + 8 (lane >> 4), chunk bit = (lane >> 3) & 1;
+    // B operand of P V from V rows (PAGED, .trans): kv row = (lane & 7) + 8 ((lane >> 3) & 1), head-dim chunk bit = lane >> 4.
     const uint32_t qoff = fa_swz(warp * 32 + (lane & 15), lane >> 4);
     const uint32_t boff = fa_swz((lane & 7) + 8 * (lane >> 4), (lane >> 3) & 1);
+    const uint32_t voff = fa_swz((lane & 7) + 8 * ((lane >> 3) & 1), lane >> 4);
     float o[2][HD / 8][4];
 #pragma unroll
     for (int mt = 0; mt < 2; ++mt)
@@ -204,13 +242,16 @@ __global__ void __launch_bounds__(FA_THREADS, 2) flash_prefill_kernel(const __gr
                     }
                 }
             }
-            // ---- O += P V  (B = V^T rows: head dim, kv contiguous) ---------------------------------------------
+            // ---- O += P V  (B = V^T rows: head dim, kv contiguous; PAGED: V rows, transposed by ldmatrix) ----------
 #pragma unroll
             for (int ks = 0; ks < FA_BN / 16; ++ks) {
 #pragma unroll
                 for (int np = 0; np < HD / 16; ++np) {
                     uint32_t b0, b1, b2, b3;
-                    fa_ldsm4(sv + np * (16 * 128) + (boff ^ (ks << 5)), b0, b1, b2, b3);
+                    if constexpr (PAGED)
+                        fa_ldsm4t(sv + (np >> 2) * (FA_BN * 128) + ks * (16 * 128) + (voff ^ ((np & 3) << 5)), b0, b1, b2, b3);
+                    else
+                        fa_ldsm4(sv + np * (16 * 128) + (boff ^ (ks << 5)), b0, b1, b2, b3);
 #pragma unroll
                     for (int mt = 0; mt < 2; ++mt) {
                         fa_mma(o[mt][2 * np], pa[mt][ks], b0, b1);
@@ -231,7 +272,7 @@ __global__ void __launch_bounds__(FA_THREADS, 2) flash_prefill_kernel(const __gr
             float l = lrow[mt][hh];
             l += __shfl_xor_sync(0xffffffffu, l, 1);
             l += __shfl_xor_sync(0xffffffffu, l, 2);
-            const int row = wrow0 + mt * 16 + g + 8 * hh;
+            const int row = wq0 + mt * 16 + g + 8 * hh;
             const float inv = (row < len && l > 0.f) ? 1.0f / l : 0.f;
             __half* orow = p.out + (size_t)(r0 + row) * p.qd + (size_t)h * HD + 2 * t4;
 #pragma unroll
@@ -261,8 +302,9 @@ __global__ void __launch_bounds__(256) rope_split_segs_kernel(const float* __res
         const int lp = (segs.len[i] + 127) / 128 * 128;
         if (t0 >= segs.start[i] && t0 < segs.start[i] + lp) seq = i;
     }
-    const int pos0 = seq >= 0 ? t0 - segs.start[seq] : 0;
-    const int n_valid = seq >= 0 ? max(0, min(RS_ROWS, segs.len[seq] - pos0)) : 0;      // rows pos0 .. pos0 + n_valid - 1 are tokens
+    const int rel0 = seq >= 0 ? t0 - segs.start[seq] : 0;
+    const int n_valid = seq >= 0 ? max(0, min(RS_ROWS, segs.len[seq] - rel0)) : 0;      // rows rel0 .. rel0 + n_valid - 1 are tokens
+    const int pos0 = seq >= 0 ? segs.pos0[seq] + rel0 : 0;                               // absolute position of the block's first row
     const int* page_table = seq >= 0 ? segs.table[seq] : nullptr;
     const bool cache = k_cache != nullptr && page_table != nullptr;
     for (int j = 0; j < RS_ROWS; ++j) {
@@ -309,29 +351,43 @@ __global__ void __launch_bounds__(256) rope_split_segs_kernel(const float* __res
 }  // namespace
 
 cudaError_t flash_prefill_configure() {
-    cudaError_t e = cudaFuncSetAttribute(flash_prefill_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, fa_smem_bytes<128>());
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(flash_prefill_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, fa_smem_bytes<64>());
+    cudaError_t e = cudaFuncSetAttribute(flash_prefill_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, fa_smem_bytes<128>());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(flash_prefill_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, fa_smem_bytes<64>());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(flash_prefill_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fa_smem_bytes<128>());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(flash_prefill_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fa_smem_bytes<64>());
     return e;
 }
 
 bool flash_prefill_supported(int hd) { return hd == 64 || hd == 128; }
 
 cudaError_t flash_prefill_launch(const __half* q, const __half* k, const __half* vt, __half* out, const PrefillSegs& segs, int n_head, int n_kv,
-                                 int hd, int vt_ld, float scale, cudaStream_t s) {
+                                 int hd, int vt_ld, float scale, const __half* k_cache, const __half* v_cache, cudaStream_t s) {
     if (segs.n < 1 || segs.n > PF_MAX_SEGS || !flash_prefill_supported(hd) || n_kv < 1 || n_head % n_kv || (vt_ld & 7)) return cudaErrorInvalidValue;
     int max_len = 0;
+    bool paged = false;
     for (int i = 0; i < segs.n; ++i) {
-        if (segs.len[i] < 1 || (segs.start[i] & 127)) return cudaErrorInvalidValue;     // 16-byte copies of V^T columns need aligned starts
+        if (segs.len[i] < 1 || segs.pos0[i] < 0 || (segs.start[i] & 127)) return cudaErrorInvalidValue;     // 16-byte copies of V^T columns need aligned starts
         max_len = segs.len[i] > max_len ? segs.len[i] : max_len;
+        paged = paged || segs.pos0[i] > 0;
+    }
+    if (paged) {          // every segment then reads its keys from its pages
+        if (!k_cache || !v_cache) return cudaErrorInvalidValue;
+        for (int i = 0; i < segs.n; ++i)
+            if (!segs.table[i]) return cudaErrorInvalidValue;
     }
     FlashParams p{};
-    p.q = q; p.k = k; p.vt = vt; p.out = out;
-    p.qd = n_head * hd; p.kvd = n_kv * hd; p.vt_ld = vt_ld; p.grp = n_head / n_kv;
+    p.q = q; p.k = k; p.vt = vt; p.out = out; p.k_cache = k_cache; p.v_cache = v_cache;
+    p.qd = n_head * hd; p.kvd = n_kv * hd; p.vt_ld = vt_ld; p.grp = n_head / n_kv; p.n_kv = n_kv;
     p.scale_log2 = scale * 1.4426950408889634f;
     p.segs = segs;
     const dim3 grid((unsigned)n_head, (unsigned)((max_len + FA_BM - 1) / FA_BM), (unsigned)segs.n);
-    if (hd == 128) flash_prefill_kernel<128><<<grid, FA_THREADS, fa_smem_bytes<128>(), s>>>(p);
-    else flash_prefill_kernel<64><<<grid, FA_THREADS, fa_smem_bytes<64>(), s>>>(p);
+    if (hd == 128) {
+        if (paged) flash_prefill_kernel<128, true><<<grid, FA_THREADS, fa_smem_bytes<128>(), s>>>(p);
+        else flash_prefill_kernel<128, false><<<grid, FA_THREADS, fa_smem_bytes<128>(), s>>>(p);
+    } else {
+        if (paged) flash_prefill_kernel<64, true><<<grid, FA_THREADS, fa_smem_bytes<64>(), s>>>(p);
+        else flash_prefill_kernel<64, false><<<grid, FA_THREADS, fa_smem_bytes<64>(), s>>>(p);
+    }
     return cudaGetLastError();
 }
 

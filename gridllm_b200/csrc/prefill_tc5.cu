@@ -260,13 +260,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gemm_tc5_kernel(const __grid_co
 
         // epilogue: thread = one row (the 32 lanes of a warp are 32 consecutive rows), 32 consecutive columns per chunk
         const int lr = (warp & 1) * 32 + lane, row = m0 + 64 * c + lr;
-        int pos = -1;                               // GEMM_EPI_ROPE_SPLIT: the row's position inside its sequence (-1: padding)
+        int pos = -1;                               // GEMM_EPI_ROPE_SPLIT: the row's absolute position in its sequence (-1: padding)
         const int* page_table = nullptr;
         if (p.epi == GEMM_EPI_ROPE_SPLIT) {
             for (int i = 0; i < p.rope.segs.n; ++i) {
                 const int s0 = p.rope.segs.start[i], ln = p.rope.segs.len[i];
                 if (row >= s0 && row < s0 + (ln + 127) / 128 * 128) {
-                    pos = row - s0 < ln ? row - s0 : -1;
+                    pos = row - s0 < ln ? p.rope.segs.pos0[i] + row - s0 : -1;
                     page_table = p.rope.segs.table[i];
                 }
             }

@@ -44,7 +44,7 @@ class NativeError(RuntimeError):
 class EngineOpts(C.Structure):
     _fields_ = [("max_ctx", C.c_int32), ("act_bits", C.c_int32), ("use_graph", C.c_int32), ("use_pdl", C.c_int32),
                 ("prefill_mode", C.c_int32), ("max_batch", C.c_int32), ("kv_pool_tokens", C.c_int32), ("batch_weights", C.c_int32),
-                ("reserved", C.c_int32 * 8)]
+                ("prefix_cache", C.c_int32), ("reserved", C.c_int32 * 7)]
 
 
 class ModelInfo(C.Structure):
@@ -185,7 +185,8 @@ class Engine:
     """One GGUF model resident on one GPU (gl_engine)."""
 
     def __init__(self, gguf_path: str, device: int = 0, max_ctx: int = 0, act_bits: int = 16, use_graph: bool = True,
-                 use_pdl: bool = True, prefill_mode: int = 0, max_batch: int = 0, kv_pool_tokens: int = 0, batch_weights: int = 0):
+                 use_pdl: bool = True, prefill_mode: int = 0, max_batch: int = 0, kv_pool_tokens: int = 0, batch_weights: int = 0,
+                 prefix_cache: bool = False):
         self._lib = load_library()
         self._h = C.c_void_p()
         o = EngineOpts()
@@ -193,6 +194,8 @@ class Engine:
         o.prefill_mode = prefill_mode   # 0 auto (batched tensor-core prefill), 1 sequential decode steps
         # continuous batching: sequences open at once (gl_seq_open), the KV pool they share, and which weights the batched step reads
         o.max_batch, o.kv_pool_tokens, o.batch_weights = int(max_batch), int(kv_pool_tokens), int(batch_weights)
+        # generate() keeps the KV pages of the longest prefix it shares with the previous generate() (include/gridllm_native.h)
+        o.prefix_cache = int(bool(prefix_cache))
         _check(self._lib.gl_engine_create(gguf_path.encode(), device, C.byref(o), C.byref(self._h)))
         self.info = ModelInfo()
         _check(self._lib.gl_engine_info(self._h, C.byref(self.info)))

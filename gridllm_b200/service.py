@@ -102,7 +102,12 @@ class NativeInferenceService:
         one engine and are decoded together, one batched step per token (gridllm_b200/batching.py); 0 / 1 = one request at a time.
         jinja_templates: render tokenizer.chat_template as Jinja for chat requests (default); False = family framing only.
         penalty_defaults: repetition-penalty options a request inherits when it does not carry them.  None = no penalty; pass
-        OLLAMA_PENALTY_DEFAULTS to penalise like an Ollama worker."""
+        OLLAMA_PENALTY_DEFAULTS to penalise like an Ollama worker.
+        engine_kw: further Engine options, e.g. prefix_cache=True: a request keeps the KV pages of the longest prefix it shares
+        with the previous request on the same engine (a multi-turn client that sends metadata.context back then pays for its
+        new tokens only, as with Ollama's cached prefix), and its prompt_eval_count counts the tokens it evaluated.  Off by
+        default, like the other Ollama-behaviour switches.  With max_batch > 1 the batch runner does no reuse: each sequence
+        slot owns its own pages."""
         self._sampling_defaults = dict(sampling_defaults or {})
         self._penalty_defaults = dict(penalty_defaults or {})
         # Ollama wraps the prompt of /api/generate and /v1/completions in the model's template (system + prompt as one user

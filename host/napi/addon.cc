@@ -73,6 +73,11 @@ napi_value CreateEngine(napi_env env, napi_callback_info info) {
         if (napi_get_named_property(env, argv[2], "actBits", &v) == napi_ok) napi_get_value_int32(env, v, &o.act_bits);
         if (napi_get_named_property(env, argv[2], "maxBatch", &v) == napi_ok) napi_get_value_int32(env, v, &o.max_batch);
         if (napi_get_named_property(env, argv[2], "kvPoolTokens", &v) == napi_ok) napi_get_value_int32(env, v, &o.kv_pool_tokens);
+        if (napi_get_named_property(env, argv[2], "prefixCache", &v) == napi_ok) {      // boolean (or 0 / 1)
+            bool b = false;
+            if (napi_get_value_bool(env, v, &b) == napi_ok) o.prefix_cache = b ? 1 : 0;
+            else napi_get_value_int32(env, v, &o.prefix_cache);
+        }
     }
     o.use_graph = 1;
     o.use_pdl = 1;

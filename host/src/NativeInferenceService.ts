@@ -26,10 +26,17 @@ export class NativeInferenceService {
 		(process.env.GRIDLLM_MODELS || "").split(",").filter(Boolean).map((kv) => kv.split("=") as [string, string])
 	);
 	private device = parseInt(process.env.GRIDLLM_DEVICE || "0", 10);
+	// prefixCache: a generate keeps the KV pages of the longest prefix it shares with the previous generate on the same engine
+	// (a client that sends `context` back pays for its new tokens only); off by default (include/gridllm_native.h)
+	private engineOptions: { prefixCache?: boolean };
+
+	constructor(options: { prefixCache?: boolean } = {}) {
+		this.engineOptions = { prefixCache: !!options.prefixCache };
+	}
 
 	private engine(name: string): unknown {
 		if (!this.models[name]) throw new Error(`model '${name}' not found`);
-		if (!this.engines.has(name)) this.engines.set(name, native.createEngine(this.models[name], this.device, {}));
+		if (!this.engines.has(name)) this.engines.set(name, native.createEngine(this.models[name], this.device, this.engineOptions));
 		return this.engines.get(name);
 	}
 

@@ -59,7 +59,21 @@ typedef struct gl_engine_opts {
     int32_t kv_pool_tokens;   /* tokens of KV cache shared by all open sequences; 0 = max_ctx * max(1, max_batch) */
     int32_t batch_weights;    /* batched step reads: 0 auto (the quantised weights, dequantised tile by tile inside the GEMM, when the
                                  model's types allow it; else the resident 16-bit copy), 1 the 16-bit copy, 2 the quantised weights */
-    int32_t reserved[8];
+    /* Prefix reuse across gl_generate calls (Ollama keeps the longest cached common prefix); 0 = off (every call prefills its whole
+     * prompt).  The engine records, on the host, the ids at positions [0, n_cached) whose K / V in its single-sequence pages are
+     * final after a gl_generate: the prompt, then the generated ids the device has fed (the last draw and a stop token never
+     * are).  The next gl_generate keeps the pages of r = max(0, min(L, n_prompt - 8)) positions, L = the longest common prefix
+     * of its prompt and the record, and evaluates positions [r, n_prompt) only: at least 8 prompt tokens (the minimum of the
+     * tensor-core prompt pass) always run, so the suffix takes the same kind of pass a cold call would.  A reused prefix that
+     * came from a prompt pass gives the bits of a cold call; one that reaches into generated tokens holds K / V the decode
+     * kernels wrote, and the output is then within the decode-vs-prefill tolerance of a cold call, not bit-identical.
+     * The record is cleared by gl_kv_reset and by every other call that writes the single-sequence pages or step state:
+     * gl_prefill, gl_decode_step, gl_embed of a sequence longer than 2 048 tokens, gl_sample_logits / gl_penalize_logits /
+     * gl_constrain_logits, gl_time_decode.  No reuse under the persistent decode kernel (GL_MEGA=1), nor for gl_seq_open
+     * sequences (each slot owns its pages).  With prefix_cache on, gl_gen_stats.prompt_eval_count of gl_generate counts the
+     * tokens this call evaluated (n_prompt - r) and prompt_eval_duration their device time. */
+    int32_t prefix_cache;
+    int32_t reserved[7];
 } gl_engine_opts;
 
 typedef struct gl_model_info {
@@ -263,7 +277,10 @@ int  gl_rmsnorm(gl_engine* e, const float* x, const float* w, int32_t n, float e
 int  gl_decode_step(gl_engine* e, int32_t token, float* logits, int32_t* argmax, float* logprob);
 int  gl_kv_reset(gl_engine* e);
 int  gl_position(const gl_engine* e, int32_t* pos);
-/* batched prefill of n tokens from the current position; logits of the LAST token (may be NULL) */
+/* batched prefill of n tokens from the current position; logits of the LAST token (may be NULL).  Like gl_generate, gl_seq_open
+ * and gl_embed, it takes the tensor-core prompt pass at any length up to the engine's context (passes of 4 096 rows; a pass that
+ * does not start at position 0 attends to the earlier positions through the KV pages), and a prompt prefilled in pieces gives
+ * the bits of the same prompt in one call.  Under prefill_mode 1, or fewer than 8 tokens, the tokens step through the decode kernels. */
 int  gl_prefill(gl_engine* e, const int32_t* ids, int32_t n, float* last_logits);
 /* mean device time (ms) of one decode step replayed `iters` times at context length ctx_len
  * (KV content is whatever is resident; used for the roofline line) */
