@@ -327,7 +327,10 @@ cudaError_t gemm_tc5_configure() {
 }
 
 bool gemm_tc5_supported(const GemmParams& p) {
-    // plain (un-batched, non-causal) TN GEMMs whose rows TMA can address: 16-byte aligned bases and row strides
+    // plain (un-batched, non-causal) TN GEMMs whose rows TMA can address: 16-byte aligned bases and row strides.  The epilogue's
+    // 16-byte stores need a 16-byte aligned C; SiLU stores them unconditionally, so its rows must stay aligned too (ldc % 8).
+    if ((uintptr_t)p.c % 16) return false;
+    if (p.epi == GEMM_EPI_SILU && (p.ldc % 8)) return false;
     if (p.epi == GEMM_EPI_ROPE_SPLIT) {
         const RopeSplitArgs* r = p.rope;
         if (!r || (r->hd % 32) || p.n != (r->n_head + 2 * r->n_kv) * r->hd || (p.m % 128) || (r->vt_ld & 7) || r->segs.n < 1 || r->segs.n > PF_MAX_SEGS) return false;

@@ -106,27 +106,29 @@ def test_tokens_do_not_depend_on_who_shares_the_batch(tiny128_gguf, mode):
 
 
 @pytest.mark.timeout(600)
-@pytest.mark.parametrize("mode", MODES)
-def test_large_batch_long_contexts(tiny128_gguf, mode):
+@pytest.mark.parametrize("mode,n_seq,max_batch", [pytest.param(m_, 28, 32, id=str(m_)) for m_ in MODES] +
+                         [pytest.param(m_, n_, b_, id=f"{m_}-{n_}seq") for n_, b_ in ((40, 64), (100, 128)) for m_ in MODES])
+def test_large_batch_long_contexts(tiny128_gguf, mode, n_seq, max_batch):
     """28 sequences (the 32-row bucket: two attention splits per KV head) with 300..700-token contexts (20+ KV pages per split:
-    several TMA tiles per CTA, partial merge) -- the shape of BASELINE config 3 at test size.  Spot-checked against the oracle
-    on four of them; all of them must finish, with finite logprobs."""
+    several TMA tiles per CTA, partial merge) -- the shape of BASELINE config 3 at test size.  40 sequences run bucket 64
+    (qgemm with NB = 64 under batch_weights 2) and 100 sequences bucket 128 (gemm_tc5 at m = 128 on the resident 16-bit
+    weights).  Spot-checked against the oracle on four of them; all of them must finish, with finite logprobs."""
     from oracle import llama_oracle as O
     m = O.load_gguf(tiny128_gguf)
-    e = _engine(tiny128_gguf, max_batch=32, max_ctx=1024, batch_weights=mode)
+    e = _engine(tiny128_gguf, max_batch=max_batch, max_ctx=1024, batch_weights=mode)
     rng = np.random.Generator(np.random.PCG64(2024))
-    lens = [int(x) for x in rng.integers(300, 700, size=28)]
+    lens = [int(x) for x in rng.integers(300, 700, size=n_seq)]
     prompts = [rng.integers(0, m.n_vocab - 3, size=n) for n in lens]
     slots = [e.seq_open(p, num_predict=6, ignore_eos=True) for p in prompts]
     lg = {}
     got = _drain(e, {s: 6 for s in slots}, lg)
     assert all(len(got[s][0]) == 6 and np.isfinite(got[s][1]).all() for s in slots)
-    for k in (0, 9, 17, 27):
+    for k in (0, 9, 17, n_seq - 1):
         ref = O.LlamaOracle(m, act="exact", kv_f16=True).generate(prompts[k], 6)
         assert _check_against_oracle(ref, got[slots[k]][0], got[slots[k]][1], lg[slots[k]], ("large", mode, lens[k])) >= 1
     for s in slots:
         e.seq_close(s)
-    ms, launches, wbytes = e.time_batch_step(32, 500, iters=4)
+    ms, launches, wbytes = e.time_batch_step(min(max_batch, 32), 500, iters=4)
     assert ms > 0 and launches > 0
     e.close()
 
