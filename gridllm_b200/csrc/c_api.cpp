@@ -58,8 +58,9 @@ static_assert(offsetof(gl_engine_opts, batch_weights) == 28 && offsetof(gl_engin
 
 // the format field of a generating request; nullptr when valid
 const char* check_format(const gl_sample_opts& so) {
-    if (so.format != 0 && so.format != GL_FORMAT_JSON) return "format must be 0 (off) or GL_FORMAT_JSON";
-    if (so.format == GL_FORMAT_JSON && so.ignore_eos) return "format json cannot be combined with ignore_eos: a JSON document ends on a stop token";
+    if (so.format != 0 && so.format != GL_FORMAT_JSON && so.format < GL_FORMAT_SCHEMA_BASE)
+        return "format must be 0 (off), GL_FORMAT_JSON or a gl_format_schema code";
+    if (so.format != 0 && so.ignore_eos) return "format json cannot be combined with ignore_eos: a JSON document ends on a stop token";
     return nullptr;
 }
 }  // namespace
@@ -273,8 +274,17 @@ int gl_penalize_logits(gl_engine* e, float* logits, int32_t n_vocab, const gl_sa
 int gl_constrain_logits(gl_engine* e, float* logits, int32_t n_vocab, const gl_sample_opts* opts, const int32_t* generated,
                         int32_t n_generated) {
     if (!e || !logits || !opts) return bad("gl_constrain_logits: null argument");
-    if (opts->format != 0 && opts->format != GL_FORMAT_JSON) return bad("format must be 0 (off) or GL_FORMAT_JSON");
+    if (opts->format != 0 && opts->format != GL_FORMAT_JSON && opts->format < GL_FORMAT_SCHEMA_BASE)
+        return bad("format must be 0 (off), GL_FORMAT_JSON or a gl_format_schema code");
     return ret(e->impl->constrain_logits(logits, n_vocab, *opts, generated, n_generated));
+}
+
+int gl_format_schema(gl_engine* e, const char* schema_utf8, int32_t n_bytes, int32_t* format_out) {
+    if (!e || !schema_utf8 || n_bytes < 0 || !format_out) return bad("gl_format_schema: bad argument");
+    int code = 0;
+    const int rc = ret(e->impl->format_schema(schema_utf8, n_bytes, &code));
+    if (rc == GL_OK) *format_out = code;
+    return rc;
 }
 
 int gl_gemv(gl_engine* e, int ggml_type, const void* w_host, int32_t rows, int32_t cols, const float* x, float* y, int32_t iters,

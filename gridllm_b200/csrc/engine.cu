@@ -89,6 +89,7 @@ Engine::~Engine() {
         for (auto& g : v)
             if (g) cudaGraphExecDestroy(g);
     for (auto& ev : ev_) if (ev) cudaEventDestroy(ev);
+    for (auto& kv : schemas_) cudaFree(kv.second.dev);
     for (void* p : allocs_) cudaFree(p);
     for (void* p : pf_allocs_) cudaFree(p);
     if (stream_) cudaStreamDestroy(stream_);
@@ -461,14 +462,16 @@ StepState Engine::make_state(int pos, int token, int n_prompt, int out_idx, cons
     h.presence_penalty = pen ? so->presence_penalty : 0.f;
     h.frequency_penalty = pen ? so->frequency_penalty : 0.f;
     if (penalised) *penalised = pen ? 1 : 0;
-    // JSON grammar mask (json_mask.cu): json_st starts zeroed, the automaton's initial state
-    h.json = (so && so->format == GL_FORMAT_JSON) ? 1 : 0;
+    // JSON grammar mask (json_mask.cu): json_st starts zeroed, the automaton's initial state; 2: a registered schema
+    // (schema_mask.cu), whose state lives in the sequence's SchemaSlot
+    h.json = !so ? 0 : so->format == GL_FORMAT_JSON ? 1 : so->format >= GL_FORMAT_SCHEMA_BASE ? 2 : 0;
     return h;
 }
 
 Status Engine::set_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so) {
     const StepState h = make_state(pos, token, n_prompt, out_idx, so, &sampler_, &penalised_);
     json_ = h.json;
+    if (h.json == 2) ST(schema_bind(schema_entry(), so->format));
     if (bar_counter_) CU(cudaMemsetAsync(bar_counter_, 0, 4, stream_));
     CU(cudaMemcpyAsync(st_, &h, sizeof(h), cudaMemcpyHostToDevice, stream_));
     CU(cudaStreamSynchronize(stream_));     // h is on the stack
@@ -629,7 +632,11 @@ Status Engine::enqueue_head(cudaStream_t s, bool keep_logits, int* n_launch) {
         CU(penalty_launch(pp, 1, false, s));
         ++*n_launch;
     }
-    if (json_) {               // the JSON grammar mask after the penalties, right before the draw (json_mask.cu)
+    if (json_ == 2) {          // a JSON schema: the schema mask in the JSON mask's place (schema_mask.cu)
+        SchemaMaskParams sp{logits_, n_vocab_, st_, nullptr, schema_entry(), json_tab_, json_off_, json_bytes_, json_cls_};
+        CU(schema_mask_launch(sp, 1, false, s));
+        ++*n_launch;
+    } else if (json_) {        // the JSON grammar mask after the penalties, right before the draw (json_mask.cu)
         JsonMaskParams jp{logits_, n_vocab_, st_, nullptr, json_off_, json_bytes_, json_cls_};
         CU(json_mask_launch(jp, 1, false, s));
         ++*n_launch;
@@ -666,9 +673,9 @@ Status Engine::run_steps(int n_nohead, int n_head, bool keep_logits) {
         if (n_head > 0) ST(launch_mega(n_head, true, keep_logits));
         return {};
     }
-    // the step with a head exists in 24 captured variants (sampler x plain / logits kept x without / with the penalty kernel x
-    // without / with the JSON mask kernel); all but the first lazily
-    cudaGraphExec_t* head = &g_head_var_[sampler_][keep_logits ? 1 : 0][penalised_ ? 1 : 0][json_ ? 1 : 0];
+    // the step with a head exists in 36 captured variants (sampler x plain / logits kept x without / with the penalty kernel x
+    // without format / with the JSON mask kernel / with the schema mask kernel); all but the first lazily
+    cudaGraphExec_t* head = &g_head_var_[sampler_][keep_logits ? 1 : 0][penalised_ ? 1 : 0][json_];
     if (use_graph_ && n_head > 0 && !*head) {
         cudaGraph_t g = nullptr;
         CU(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
@@ -1064,10 +1071,16 @@ bool Engine::json_stop(const gl_sample_opts& so, int32_t id) const {
 
 Status Engine::json_admit(const gl_sample_opts& so, bool single_path) {
     if (so.format == 0) return {};
-    if (so.format != GL_FORMAT_JSON) return fail(GL_ERR_INVALID, "format must be 0 (off) or GL_FORMAT_JSON");
+    const bool schema = so.format >= GL_FORMAT_SCHEMA_BASE;
+    if (so.format != GL_FORMAT_JSON && !schema) return fail(GL_ERR_INVALID, "format must be 0 (off), GL_FORMAT_JSON or a gl_format_schema code");
+    if (schema && !schemas_.count(so.format)) return fail(GL_ERR_INVALID, "format: unknown or evicted schema code " + std::to_string(so.format));
     if (so.ignore_eos) return fail(GL_ERR_INVALID, "format json cannot be combined with ignore_eos: a JSON document ends on a stop token");
     if (single_path && use_mega_) return fail(GL_ERR_UNSUPPORTED, "the persistent decode kernel (GL_MEGA=1) has no JSON grammar mask");
     ST(ensure_json());
+    if (schema) {
+        ST(ensure_schema_state());
+        schemas_[so.format].used = ++schema_clock_;
+    }
     // a stop id that is an ordinary token would be masked wherever it is needed, and the vocabulary guarantee would not hold
     for (int i = 0; i < so.n_stop_ids; ++i) {
         const int32_t id = so.stop_ids ? so.stop_ids[i] : -1;
@@ -1092,11 +1105,21 @@ Status Engine::constrain_logits(float* logits, int n_vocab, const gl_sample_opts
     ST(json_admit(o, false));
     // the history must be a prefix the mask allows: no stop token (it would have ended the output), no control token, every
     // byte accepted
+    const bool schema = o.format >= GL_FORMAT_SCHEMA_BASE;
     JsonState hs{};
+    SchemaState ss;
+    SchemaView sv{};
+    SchemaArrayFrames sf{ss.fr};
+    if (schema) {
+        sv = schema_view(schemas_[o.format].blob.data());
+        schema_init(ss.js, ss.cur, sv);
+    }
     for (int i = 0; i < n_generated; ++i) {
         const int32_t t = generated[i];
         const uint32_t a = json_hoff_[t], b = json_hoff_[t + 1];
-        if (json_stop(o, t) || a == b || !json_run(hs, json_hbytes_.data() + a, (int)(b - a)))
+        const bool ok = schema ? schema_run(sv, ss.js, ss.cur, sf, json_hbytes_.data() + a, (int)(b - a))
+                               : json_run(hs, json_hbytes_.data() + a, (int)(b - a));
+        if (json_stop(o, t) || a == b || !ok)
             return fail(GL_ERR_INVALID, "format json: the history is not a prefix the grammar allows (token " + std::to_string(i) + ")");
     }
     ST(kv_reset());
@@ -1106,9 +1129,14 @@ Status Engine::constrain_logits(float* logits, int n_vocab, const gl_sample_opts
     Status rs;
     do {
         cudaError_t ce = hist ? cudaMemcpyAsync(hist, generated, (size_t)n_generated * 4, cudaMemcpyHostToDevice, stream_) : cudaSuccess;
-        if (ce == cudaSuccess && hist) ce = json_replay_launch(st_, hist, n_generated, json_off_, json_bytes_, stream_);
+        if (ce == cudaSuccess && hist)
+            ce = schema ? schema_replay_launch(sch_, hist, n_generated, json_off_, json_bytes_, stream_)
+                        : json_replay_launch(st_, hist, n_generated, json_off_, json_bytes_, stream_);
         if (ce == cudaSuccess) ce = cudaMemcpyAsync(logits_, logits, (size_t)n_vocab_ * 4, cudaMemcpyHostToDevice, stream_);
-        if (ce == cudaSuccess) {
+        if (ce == cudaSuccess && schema) {
+            SchemaMaskParams sp{logits_, n_vocab_, st_, nullptr, sch_, json_tab_, json_off_, json_bytes_, json_cls_};
+            ce = schema_mask_launch(sp, 1, false, stream_);
+        } else if (ce == cudaSuccess) {
             JsonMaskParams jp{logits_, n_vocab_, st_, nullptr, json_off_, json_bytes_, json_cls_};
             ce = json_mask_launch(jp, 1, false, stream_);
         }
@@ -1119,6 +1147,93 @@ Status Engine::constrain_logits(float* logits, int n_vocab, const gl_sample_opts
     if (hist) cudaFree(hist);
     ST(rs);
     return kv_reset();
+}
+
+// ---- JSON schemas (schema_compile.cpp, schema_mask.cu) ---------------------------------------------------------------------
+Status Engine::ensure_schema_state() {
+    if (sch_) return {};
+    std::vector<uint8_t> blob;
+    std::string err;
+    static const char kAnyObject[] = "{\"type\":\"object\"}";
+    if (schema_compile(kAnyObject, sizeof kAnyObject - 1, blob, err) != GL_OK) return fail(GL_ERR_INVALID, err);
+    SchemaSlot* d = nullptr;
+    uint8_t* t = nullptr;
+    const size_t bytes = sizeof(SchemaSlot) * (1 + MAX_BATCH);
+    CU(cudaMalloc((void**)&d, bytes));
+    allocs_.push_back(d);
+    CU(cudaMalloc((void**)&t, blob.size()));
+    allocs_.push_back(t);
+    CU(cudaMemset(d, 0, bytes));
+    CU(cudaMemcpy(t, blob.data(), blob.size(), cudaMemcpyHostToDevice));
+    sch_ = d;
+    json_tab_ = t;
+    return {};
+}
+
+SchemaSlot* Engine::schema_entry() const {
+    return (bst_ && st_ >= bst_ && st_ < bst_ + MAX_BATCH) ? sch_ + 1 + (st_ - bst_) : sch_;
+}
+
+Status Engine::schema_bind(SchemaSlot* e, int code) {
+    auto it = schemas_.find(code);
+    if (it == schemas_.end() || !e) return fail(GL_ERR_INVALID, "format: unknown or evicted schema code " + std::to_string(code));
+    CU(cudaMemcpyAsync(&e->tab, &it->second.dev, sizeof(it->second.dev), cudaMemcpyHostToDevice, stream_));
+    CU(cudaStreamSynchronize(stream_));
+    return {};
+}
+
+// Compile and register a schema: identical text gives the code it got before.  The vocabulary must carry a single-byte token
+// for every byte of the keys and enum members (beside what ensure_json asks), so that a literal can always be continued.
+Status Engine::format_schema(const char* text, int n, int* code) {
+    CU(cudaSetDevice(device_));
+    if (!text || n < 0 || !code) return fail(GL_ERR_INVALID, "gl_format_schema: bad argument");
+    const std::string key(text, (size_t)n);
+    auto hit = schema_codes_.find(key);
+    if (hit != schema_codes_.end()) {
+        schemas_[hit->second].used = ++schema_clock_;
+        *code = hit->second;
+        return {};
+    }
+    SchemaEntry en;
+    en.text = key;
+    std::string err;
+    const int rc = schema_compile(text, (size_t)n, en.blob, err);
+    if (rc != GL_OK) return fail(rc, err);
+    ST(ensure_json());
+    bool single[256] = {};
+    for (int t = 0; t < n_vocab_; ++t)
+        if (json_hoff_[t + 1] - json_hoff_[t] == 1 && t != tok_.eos && t != tok_.eot) single[json_hbytes_[json_hoff_[t]]] = true;
+    const SchemaHeader* h = reinterpret_cast<const SchemaHeader*>(en.blob.data());
+    const uint32_t* lo = reinterpret_cast<const uint32_t*>(en.blob.data() + h->off_lit_off);
+    for (uint32_t i = h->off_lit; i < h->off_lit + lo[h->n_lits]; ++i)
+        if (!single[en.blob[i]]) {
+            char buf[8];
+            snprintf(buf, sizeof buf, "0x%02X", en.blob[i]);
+            return fail(GL_ERR_UNSUPPORTED, std::string("format schema: the vocabulary has no single-byte token for byte ") + buf +
+                                                " of a key or enum member, so a continuation cannot be guaranteed");
+        }
+    if ((int)schemas_.size() >= SCHEMA_CACHE) {                 // evict the least recently used schema no open sequence uses
+        int victim = -1;
+        uint64_t oldest = UINT64_MAX;
+        for (auto& kv : schemas_) {
+            bool in_use = false;
+            for (auto& S : slots_) in_use = in_use || (S.open && S.schema == kv.first);
+            if (!in_use && kv.second.used < oldest) { oldest = kv.second.used; victim = kv.first; }
+        }
+        if (victim < 0) return fail(GL_ERR_NOMEM, "format schema: all 64 registered schemas are in use by open sequences");
+        cudaFree(schemas_[victim].dev);
+        schema_codes_.erase(schemas_[victim].text);
+        schemas_.erase(victim);
+    }
+    CU(cudaMalloc((void**)&en.dev, en.blob.size()));
+    const cudaError_t ce = cudaMemcpy(en.dev, en.blob.data(), en.blob.size(), cudaMemcpyHostToDevice);
+    if (ce != cudaSuccess) { cudaFree(en.dev); CU(ce); }
+    en.used = ++schema_clock_;
+    const int c = next_schema_++;
+    schema_codes_[key] = c;
+    schemas_[c] = std::move(en);
+    *code = c;
+    return {};
 }
 
 Status Engine::decode_step(int token, float* logits, int* argmax, float* logprob) {

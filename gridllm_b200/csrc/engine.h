@@ -5,6 +5,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <map>
 #include <memory>
 #include <string>
 #include <vector>
@@ -211,7 +212,7 @@ private:
     struct SeqSlot {
         bool open = false, done = false, first_pending = false;
         std::vector<int> pages;
-        int n_prompt = 0, n_pred = 0, produced = 0, sampler = 0, penalised = 0, json = 0;
+        int n_prompt = 0, n_pred = 0, produced = 0, sampler = 0, penalised = 0, json = 0, schema = 0;     // schema: its format code
         int32_t last_token = 0;
         float first_lp = 0.f;
         int last_row = -1;                            // row of the last batched step this sequence took part in
@@ -250,13 +251,17 @@ private:
     Status pack_qgemm(const std::vector<const GGUFTensor*>& src, int mode, QGemmWeights& out, uint8_t*& tmp, size_t& tmp_cap);
     // [bucket][variant]: variant bit 0 the penalty kernel (steps in which some row has penalties), bit 1 the JSON mask kernel
     // (steps in which some row has format json)
-    cudaGraphExec_t g_batch_[N_BUCKETS][4] = {};
+    // bit 2 the schema mask kernel (steps in which some row has a schema; it also masks the format json rows, so bit 1 is
+    // then clear)
+    cudaGraphExec_t g_batch_[N_BUCKETS][8] = {};
     int batch_launches_ = 0;                          // kernels of one batched step (without the penalty / JSON mask kernels)
     uint64_t bc_[8] = {};                             // gl_batch_counters
     Status ensure_batch_state();
     Status seq_open_single(const int32_t* prompt, int n_prompt, const gl_sample_opts& so, int* slot);
-    Status enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bool json, int* n_launch);
-    Status run_batch_graph(int bucket, bool penalised, bool json);
+    Status enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bool json, int* n_launch, bool schema = false);
+    Status run_batch_graph(int bucket, bool penalised, bool json, bool schema = false);
+    cudaError_t batch_schema_launch(int bucket, cudaStream_t s);
+    bool batch_schema_checked_ = false;               // the batched schema mask launch has run once outside stream capture
     cudaError_t batch_penalty_launch(int bucket, cudaStream_t s);
     cudaError_t batch_json_launch(int bucket, cudaStream_t s);
     bool batch_json_checked_ = false;                 // the batched mask launch has run once outside stream capture
@@ -266,9 +271,10 @@ private:
     static int bucket_index(int bucket) { int i = 0; while ((8 << i) < bucket) ++i; return i; }
 
     cudaGraphExec_t g_nohead_ = nullptr;
-    cudaGraphExec_t g_head_var_[3][2][2][2] = {};   // [sampler of the running request][logits kept][repetition penalties][format json]
+    cudaGraphExec_t g_head_var_[3][2][2][3] = {};   // [sampler of the running request][logits kept][repetition penalties][json_]
     int penalised_ = 0;                        // the running request has penalties: penalty.cu runs between the lm_head and the sampler
-    int json_ = 0;                             // the running request has format json: json_mask.cu runs right before the sampler
+    int json_ = 0;                             // the running request has format json (1: json_mask.cu runs right before the sampler)
+                                               // or a schema (2: schema_mask.cu does)
     // JSON grammar mask (json_mask.cu): the vocabulary's pieces on the device, built at the first JSON request (nothing before)
     uint32_t* json_off_ = nullptr;             // [n_vocab + 1] byte offsets
     uint8_t* json_bytes_ = nullptr;            // pieces back to back
@@ -281,6 +287,23 @@ private:
     // a request's format field: GL_ERR_UNSUPPORTED / GL_ERR_INVALID when the engine cannot honour it (table built on first use)
     Status json_admit(const gl_sample_opts& so, bool single_path);
     bool json_stop(const gl_sample_opts& so, int32_t id) const;     // id is a stop token of a request with these options
+    // JSON schemas (gl_format_schema; schema_mask.cu): at most SCHEMA_CACHE compiled schemas by code, least recently used
+    // evicted first unless an open sequence uses it; codes are never reused
+    static constexpr int SCHEMA_CACHE = 64;
+    struct SchemaEntry { std::string text; std::vector<uint8_t> blob; uint8_t* dev = nullptr; uint64_t used = 0; };
+    std::map<int, SchemaEntry> schemas_;
+    std::map<std::string, int> schema_codes_;
+    int next_schema_ = GL_FORMAT_SCHEMA_BASE;
+    uint64_t schema_clock_ = 0;
+    // per-sequence schema state, allocated at the first schema request: [0] the single-sequence path, [1 + slot] batch slots
+    SchemaSlot* sch_ = nullptr;
+    uint8_t* json_tab_ = nullptr;              // the built-in any-object schema (format json rows in a schema mask launch)
+    Status ensure_schema_state();
+    SchemaSlot* schema_entry() const;          // the entry of the sequence whose step state st_ points at
+    Status schema_bind(SchemaSlot* e, int code);     // e follows schema `code` from its next output 0
+public:
+    Status format_schema(const char* text, int n, int* code);
+private:
     // The top-k samplers are launched WITHOUT programmatic dependent launch: their CTAs (33 KB of shared memory each) resident
     // beside the lm_head CTAs cost the step 60 us (run 67: 1.537 -> 1.478 ms/token at top_k 40); the greedy sampler keeps it.
     bool sampler_pdl_ = false;

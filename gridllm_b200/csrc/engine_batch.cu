@@ -223,6 +223,13 @@ cudaError_t Engine::batch_json_launch(int bucket, cudaStream_t s) {
     return json_mask_launch(jp, bucket, false, s);
 }
 
+// the schema mask over the rows of a batched step: rows with a schema follow their SchemaSlot, rows with format json the
+// built-in any-object schema (the JSON mask's result); other rows leave at once
+cudaError_t Engine::batch_schema_launch(int bucket, cudaStream_t s) {
+    SchemaMaskParams sp{blogits_, n_vocab_, bst_, bctl_, sch_ + 1, json_tab_, json_off_, json_bytes_, json_cls_};
+    return schema_mask_launch(sp, bucket, false, s);
+}
+
 // Prefill a prompt into a free slot's own pages and draw its first token.  The single-sequence code runs unchanged on the
 // slot's state: the members it reads (page table, step state, output buffers) point at the slot's rows for the duration.
 // One prompt.  It takes the SAME path as a prompt opened together with others (gl_seq_open_many with one entry: packed prompt
@@ -316,7 +323,8 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
     }
     S.open = true;
     S.n_prompt = n_prompt; S.n_pred = n_pred; S.produced = 0; S.sampler = sampler; S.penalised = penalised; S.first_pending = true;
-    S.json = so.format == GL_FORMAT_JSON ? 1 : 0;
+    S.json = so.format == GL_FORMAT_JSON ? 1 : so.format >= GL_FORMAT_SCHEMA_BASE ? 2 : 0;
+    S.schema = S.json == 2 ? so.format : 0;
     S.t_open_ns = t_open; S.launches = prefill_launches; S.stopped = S.done;
     bc_[3] += (uint64_t)S.prefill_ns; bc_[4] += (uint64_t)n_prompt; bc_[5] += 1; bc_[6] += (uint64_t)prefill_launches;
     *slot_out = slot;
@@ -426,7 +434,7 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             std::vector<StepState> hst(P);
             BatchCtl hc{};
             hc.n_rows = P;
-            bool any_pen = false, any_json = false;
+            bool any_pen = false, any_json = false, any_schema = false;
             for (int i = 0; i < P && ce == cudaSuccess; ++i) {
                 const int w = which[i], n = lens[i];
                 int sampler = 0, pen = 0;
@@ -434,7 +442,13 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
                 slots_[pslots[i]].sampler = sampler;
                 slots_[pslots[i]].penalised = pen;
                 slots_[pslots[i]].json = hst[i].json;
+                slots_[pslots[i]].schema = hst[i].json == 2 ? opts[w].format : 0;
                 any_json = any_json || hst[i].json != 0;
+                any_schema = any_schema || hst[i].json == 2;
+                if (hst[i].json == 2) {
+                    Status bs = schema_bind(sch_ + 1 + pslots[i], opts[w].format);
+                    if (!bs.ok()) { rs = bs; break; }
+                }
                 if (pen) {                                   // the head of the history the penalty kernel reads
                     Status ks = keep_prompt(pslots[i], ids + offs[w], n);
                     if (!ks.ok()) { rs = ks; break; }
@@ -451,8 +465,8 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
                 ce = batch_penalty_launch(bucket, stream_);
                 ++launches;
             }
-            if (ce == cudaSuccess && any_json) {             // then the JSON grammar mask of the rows that have it
-                ce = batch_json_launch(bucket, stream_);
+            if (ce == cudaSuccess && any_json) {             // then the JSON grammar mask of the rows that have it (the schema mask
+                ce = any_schema ? batch_schema_launch(bucket, stream_) : batch_json_launch(bucket, stream_);      // when some row has a schema)
                 ++launches;
             }
             if (ce == cudaSuccess) ce = batch_sample_greedy_launch(blogits_, n_vocab_, bucket, bctl_, bst_, bout_ids_, bout_lp_, max_out_, bsample_scratch_, stream_);
@@ -546,7 +560,7 @@ Status Engine::seq_logits(int slot, float* out, int n_vocab) {
 }
 
 // every launch of one batched step, for `bucket` rows; all pointers are fixed, the composition is read from bctl_ / bst_
-Status Engine::enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bool json, int* n_launch) {
+Status Engine::enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bool json, int* n_launch, bool schema) {
     const int qd = n_head_ * hd_, kvd = n_kv_ * hd_, ldq = qd + 2 * kvd;
     const float scale = 1.0f / std::sqrt((float)hd_);
     int nl = 0;
@@ -633,6 +647,9 @@ Status Engine::enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bo
     // then the JSON grammar mask of the rows that have format json (json_mask.cu): only in the variants used for steps in which
     // some row has it
     if (json) { CU(batch_json_launch(bucket, s)); ++nl; }
+    // or the schema mask, for the rows with a schema and those with format json alike (schema_mask.cu): only in the variants
+    // used for steps in which some row has a schema
+    if (schema) { CU(batch_schema_launch(bucket, s)); ++nl; }
     CU(batch_sample_greedy_launch(blogits_, n_vocab_, bucket, bctl_, bst_, bout_ids_, bout_lp_, max_out_, bsample_scratch_, s)); ++nl;
     if (n_launch) *n_launch = nl;
     return {};
@@ -640,25 +657,26 @@ Status Engine::enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bo
 
 // penalised / json: the variants with the penalty kernel / the JSON mask kernel (up to four captured steps per bucket);
 // batch_launches_ counts the plain one
-Status Engine::run_batch_graph(int bucket, bool penalised, bool json) {
+Status Engine::run_batch_graph(int bucket, bool penalised, bool json, bool schema) {
     const int bi = bucket_index(bucket);
     if (penalised && !bpen_counts_) return failb(GL_ERR_INVALID, "batched step: no penalty state");
     if (json && !json_off_) return failb(GL_ERR_INVALID, "batched step: no JSON vocabulary table");
-    const int extra = (penalised ? 1 : 0) + (json ? 1 : 0);
+    if (schema && !sch_) return failb(GL_ERR_INVALID, "batched step: no schema state");
+    const int extra = (penalised ? 1 : 0) + (json ? 1 : 0) + (schema ? 1 : 0);
     if (!use_graph_) {
         int nl = 0;
-        ST(enqueue_batch_step(stream_, bucket, penalised, json, &nl));
+        ST(enqueue_batch_step(stream_, bucket, penalised, json, &nl, schema));
         batch_launches_ = nl - extra;
         return {};
     }
-    cudaGraphExec_t& ge = g_batch_[bi][(penalised ? 1 : 0) | (json ? 2 : 0)];
+    cudaGraphExec_t& ge = g_batch_[bi][(penalised ? 1 : 0) | (json ? 2 : 0) | (schema ? 4 : 0)];
     if (!ge) {
-        if (json && !batch_json_checked_) {
+        if ((json && !batch_json_checked_) || (schema && !batch_schema_checked_)) {
             // one un-captured launch on a composition of no rows (every CTA leaves at once; a launch on the real rows would
             // advance their automata) validates the configuration outside stream capture; the step's composition is restored
             BatchCtl none{};
             CU(cudaMemcpyAsync(bctl_, &none, sizeof(int), cudaMemcpyHostToDevice, stream_));
-            cudaError_t e0 = batch_json_launch(8, stream_);
+            cudaError_t e0 = json ? batch_json_launch(8, stream_) : batch_schema_launch(8, stream_);
             if (e0 == cudaSuccess) e0 = cudaStreamSynchronize(stream_);
             BatchCtl h{};
             h.n_rows = (int)last_rows_.size();
@@ -666,12 +684,12 @@ Status Engine::run_batch_graph(int bucket, bool penalised, bool json) {
             CU(cudaMemcpyAsync(bctl_, &h, sizeof(h), cudaMemcpyHostToDevice, stream_));
             CU(cudaStreamSynchronize(stream_));                       // h is on the stack
             CU(e0);
-            batch_json_checked_ = true;
+            (json ? batch_json_checked_ : batch_schema_checked_) = true;
         }
         cudaGraph_t g = nullptr;
         int nl = 0;
         CU(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
-        Status st = enqueue_batch_step(stream_, bucket, penalised, json, &nl);
+        Status st = enqueue_batch_step(stream_, bucket, penalised, json, &nl, schema);
         cudaError_t e = cudaStreamEndCapture(stream_, &g);
         if (!st.ok()) { if (g) cudaGraphDestroy(g); return st; }
         if (e != cudaSuccess) return failb(GL_ERR_CUDA, std::string("batched step: graph capture: ") + cudaGetErrorString(e));
@@ -731,14 +749,16 @@ Status Engine::batch_step(int32_t* out_slots, int32_t* out_ids, float* out_lps, 
         last_rows_ = rows;
     }
     last_bucket_ = bucket;
-    bool penalised = false, json = false;            // the step with the penalty / JSON mask kernel only when some row needs it
+    bool penalised = false, json = false, schema = false;     // the step with the penalty / a mask kernel only when some row needs it
     for (int r = 0; r < B; ++r) {
         penalised = penalised || slots_[rows[r]].penalised != 0;
         json = json || slots_[rows[r]].json != 0;
+        schema = schema || slots_[rows[r]].json == 2;
     }
+    if (schema) json = false;                        // the schema mask masks the format json rows too
     CU(cudaEventRecord(ev_[2], stream_));
-    ST(run_batch_graph(bucket, penalised, json));
-    const int step_launches = batch_launches_ + (penalised ? 1 : 0) + (json ? 1 : 0) + 1;
+    ST(run_batch_graph(bucket, penalised, json, schema));
+    const int step_launches = batch_launches_ + (penalised ? 1 : 0) + (json || schema ? 1 : 0) + 1;
     for (int r = 0; r < B; ++r) {                    // sampled rows: the seeded top-k / top-p sampler of the single-sequence path
         const int slot = rows[r];
         if (slots_[slot].sampler == 0) continue;

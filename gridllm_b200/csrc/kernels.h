@@ -5,6 +5,7 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "schema_fsm.h"
 
 namespace gl {
 
@@ -181,6 +182,30 @@ cudaError_t json_mask_launch(const JsonMaskParams& p, int rows, bool pdl, cudaSt
 // one thread: the automaton from the initial state through the pieces of ids[0..n-1) (all but the last), stored as the entry
 // the mask kernel of output n reads; that kernel then advances by ids[n-1] (= st->token) itself.  gl_constrain_logits.
 cudaError_t json_replay_launch(StepState* st, const int* ids, int n, const uint32_t* offsets, const uint8_t* bytes, cudaStream_t s);
+
+// JSON schema mask (schema_mask.cu; language in schema_fsm.h, semantics in include/gridllm_native.h gl_format_schema): the grid
+// of json_mask_launch.  Rows with StepState.json = 2 follow their SchemaSlot; rows with json = 1 (format json) follow the
+// built-in any-object schema from their json_st, giving json_mask_launch's mask; other rows and finished rows leave at once.
+struct SchemaSlot {
+    const uint8_t* tab;         // the row's compiled schema (schema_compile.cpp blob), set by the host when the request starts
+    uint32_t pad[2];
+    SchemaState st[2];          // st[i & 1]: the automaton state after the output's first i tokens (as StepState.json_st)
+};
+struct SchemaMaskParams {
+    float* logits;              // row r at logits + r * n_vocab
+    int n_vocab;
+    StepState* st;              // ctl == null: the one sequence's state; else [slots]
+    const BatchCtl* ctl;        // batched step: row -> slot; null: one row
+    SchemaSlot* ss;             // ctl == null: the one sequence's entry; else [slots]
+    const uint8_t* json_tab;    // the built-in any-object schema
+    const uint32_t* offsets;    // the vocabulary table of JsonMaskParams
+    const uint8_t* bytes;
+    const uint8_t* cls;
+};
+cudaError_t schema_mask_launch(const SchemaMaskParams& p, int rows, bool pdl, cudaStream_t s);
+// one thread: e's automaton from the initial state through the pieces of ids[0..n-1), stored as entry (n - 1) & 1 (the mask
+// kernel of output n advances by ids[n-1] itself).  gl_constrain_logits.
+cudaError_t schema_replay_launch(SchemaSlot* e, const int* ids, int n, const uint32_t* offsets, const uint8_t* bytes, cudaStream_t s);
 
 // standalone pieces (used for fp-weight models and as unfused cross-checks)
 cudaError_t rmsnorm_launch(const float* x, const float* w, int n, float eps, float* y, cudaStream_t s);

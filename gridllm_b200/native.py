@@ -7,6 +7,7 @@ every entry point raises ``NativeError``.
 from __future__ import annotations
 
 import ctypes as C
+import json
 import os
 from dataclasses import dataclass
 from typing import Callable, List, Optional, Sequence
@@ -27,7 +28,7 @@ STATUS_NAMES = {0: "GL_OK", -1: "GL_ERR_INVALID", -2: "GL_ERR_IO", -3: "GL_ERR_F
 ABI_SYMBOLS = [
     "gl_abi_version", "gl_last_error", "gl_device_count", "gl_engine_create", "gl_engine_destroy",
     "gl_engine_info", "gl_tokenize", "gl_detokenize", "gl_chat_template", "gl_generate", "gl_embed", "gl_last_logits", "gl_sample_logits",
-    "gl_penalize_logits", "gl_constrain_logits",
+    "gl_penalize_logits", "gl_constrain_logits", "gl_format_schema",
     "gl_seq_open", "gl_seq_open_many", "gl_batch_step", "gl_seq_close", "gl_seq_logits", "gl_seq_stats", "gl_token_piece", "gl_token_text", "gl_batch_counters", "gl_time_batch_step",
     "gl_gemv", "gl_gemv_model_tensor", "gl_rmsnorm", "gl_decode_step", "gl_kv_reset", "gl_position",
     "gl_prefill", "gl_time_decode",
@@ -74,6 +75,7 @@ class SampleOpts(C.Structure):
 
 
 GL_FORMAT_JSON = 1
+GL_FORMAT_SCHEMA_BASE = 256     # gl_format_schema codes start here
 
 
 def _format_code(fmt) -> int:
@@ -133,6 +135,7 @@ def load_library() -> C.CDLL:
     lib.gl_sample_logits.argtypes = [vp, f32p, i32, C.POINTER(SampleOpts), i32, i32p, f32p]
     lib.gl_penalize_logits.argtypes = [vp, f32p, i32, C.POINTER(SampleOpts), i32p, i32]
     lib.gl_constrain_logits.argtypes = [vp, f32p, i32, C.POINTER(SampleOpts), i32p, i32]
+    lib.gl_format_schema.argtypes = [vp, C.c_char_p, i32, i32p]
     lib.gl_seq_open.argtypes = [vp, i32p, i32, C.POINTER(SampleOpts), i32p]
     lib.gl_seq_open_many.argtypes = [vp, i32p, i32p, i32, C.POINTER(SampleOpts), i32p, i32p]
     lib.gl_batch_step.argtypes = [vp, i32p, i32p, f32p, i32p, i32, i32p]
@@ -249,7 +252,7 @@ class Engine:
         p = np.ascontiguousarray(prompt, dtype=np.int32)
         so = SampleOpts()
         so.num_predict, so.ignore_eos, so.want_logits = num_predict, int(ignore_eos), int(want_logits)
-        so.format = _format_code(format)
+        so.format = self._format(format)
         so.temperature, so.top_k, so.top_p, so.seed = float(temperature), int(top_k), float(top_p), int(seed) & (2**64 - 1)
         _set_penalties(so, dict(repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n, presence_penalty=presence_penalty,
                                 frequency_penalty=frequency_penalty, min_p=min_p))
@@ -281,7 +284,7 @@ class Engine:
         p = np.ascontiguousarray(prompt, dtype=np.int32)
         so = SampleOpts()
         so.num_predict, so.ignore_eos = (num_predict if num_predict > 0 else 128), int(ignore_eos)
-        so.format = _format_code(format)
+        so.format = self._format(format)
         so.temperature, so.top_k, so.top_p, so.seed = float(temperature), int(top_k), float(top_p), int(seed) & (2**64 - 1)
         _set_penalties(so, dict(repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n, presence_penalty=presence_penalty,
                                 frequency_penalty=frequency_penalty, min_p=min_p))
@@ -308,7 +311,7 @@ class Engine:
             so[i].temperature, so[i].top_k, so[i].top_p = float(o.get("temperature", 0.0)), int(o.get("top_k", 0)), float(o.get("top_p", 1.0))
             so[i].seed = int(o.get("seed", 0)) & (2**64 - 1)
             _set_penalties(so[i], {k: o.get(k) for k in PENALTY_DEFAULTS})
-            so[i].format = _format_code(o.get("format"))
+            so[i].format = self._format(o.get("format"))
             stops = np.ascontiguousarray(o.get("stop_ids", ()), dtype=np.int32)
             keep.append(stops)
             so[i].n_stop_ids = len(stops)
@@ -399,12 +402,33 @@ class Engine:
         g = np.ascontiguousarray(generated, dtype=np.int32)
         so = SampleOpts()
         so.num_predict = 1
-        so.format = _format_code(format)
+        so.format = self._format(format)
         stops = np.ascontiguousarray(stop_ids, dtype=np.int32)
         so.n_stop_ids = len(stops)
         so.stop_ids = _i32p(stops) if len(stops) else None
         _check(self._lib.gl_constrain_logits(self._h, _f32p(out), len(out), C.byref(so), _i32p(g) if len(g) else None, len(g)))
         return out
+
+    def format_schema(self, schema) -> int:
+        """Compile and register a JSON schema (gl_format_schema): its code for `format=`.  A dict is serialised compactly with
+        its key order kept; a str / bytes is taken as it is.  Identical text gives the same code.  NativeError GL_ERR_INVALID
+        for malformed JSON, GL_ERR_UNSUPPORTED for a schema outside the subset (the message names the keyword and its
+        JSON pointer)."""
+        if isinstance(schema, dict):
+            schema = json.dumps(schema, ensure_ascii=False, separators=(",", ":"))
+        raw = schema.encode("utf-8") if isinstance(schema, str) else bytes(schema)
+        code = C.c_int32(0)
+        _check(self._lib.gl_format_schema(self._h, raw, len(raw), C.byref(code)))
+        return int(code.value)
+
+    def _format(self, fmt) -> int:
+        """the `format` keyword: None / "" / 0 off, "json" the JSON grammar mask, a dict a JSON schema (compiled through the
+        engine's cache), or a code from format_schema"""
+        if isinstance(fmt, dict):
+            return self.format_schema(fmt)
+        if isinstance(fmt, int) and not isinstance(fmt, bool) and fmt >= GL_FORMAT_SCHEMA_BASE:
+            return fmt
+        return _format_code(fmt)
 
     def last_logits(self, step: int) -> np.ndarray:
         out = np.empty(self.info.n_vocab, dtype=np.float32)

@@ -92,7 +92,8 @@ class NativeInferenceService:
 
     def __init__(self, models: Dict[str, str], device: int = 0, max_ctx: int = 0,
                  sampling_defaults: Optional[Dict[str, Any]] = None, apply_template: bool = False, max_batch: int = 0,
-                 jinja_templates: bool = True, penalty_defaults: Optional[Dict[str, Any]] = None, **engine_kw):
+                 jinja_templates: bool = True, penalty_defaults: Optional[Dict[str, Any]] = None, json_schema: bool = False,
+                 **engine_kw):
         """models: Ollama-style model name -> GGUF path.
         sampling_defaults: options a request inherits when it does not carry them.  None = greedy (temperature 0, the
         BASELINE.json configuration); pass OLLAMA_SAMPLING_DEFAULTS to behave like an Ollama worker for such requests.
@@ -103,6 +104,9 @@ class NativeInferenceService:
         jinja_templates: render tokenizer.chat_template as Jinja for chat requests (default); False = family framing only.
         penalty_defaults: repetition-penalty options a request inherits when it does not carry them.  None = no penalty; pass
         OLLAMA_PENALTY_DEFAULTS to penalise like an Ollama worker.
+        json_schema: enforce a JSON-schema `format` (metadata.format or options.format) on the GPU: the response is a document
+        of the schema, and a schema outside the supported subset fails the request before it runs.  False (default): a schema
+        object only asks for valid JSON of any shape.
         engine_kw: further Engine options, e.g. prefix_cache=True: a request keeps the KV pages of the longest prefix it shares
         with the previous request on the same engine (a multi-turn client that sends metadata.context back then pays for its
         new tokens only, as with Ollama's cached prefix), and its prompt_eval_count counts the tokens it evaluated.  Off by
@@ -110,6 +114,7 @@ class NativeInferenceService:
         slot owns its own pages."""
         self._sampling_defaults = dict(sampling_defaults or {})
         self._penalty_defaults = dict(penalty_defaults or {})
+        self._json_schema = bool(json_schema)
         # Ollama wraps the prompt of /api/generate and /v1/completions in the model's template (system + prompt as one user
         # turn) unless the request says raw [external]; off by default: the prompt text is tokenised as it is
         self._apply_template = bool(apply_template)
@@ -337,6 +342,14 @@ class NativeInferenceService:
         ignore_eos = bool(options.get("ignore_eos", False))
         if fmt and ignore_eos:
             raise RuntimeError("format json cannot be combined with ignore_eos: a JSON document ends on a stop token")
+        if fmt and isinstance(fmt.get("format"), dict):
+            # a schema outside the subset fails the request before it runs; the engine keeps the compiled schema, and the
+            # generation (or the batch runner's open) finds it again by its text
+            try:
+                with self._lock:
+                    eng.format_schema(fmt["format"])
+            except N.NativeError as ex:
+                raise RuntimeError(ex.detail) from None
         # a generation that would run past the engine's context ends at it (done_reason "length") instead of failing; a prompt
         # that does not fit at all still fails (GL_ERR_CONTEXT)
         n_ctx = int(getattr(eng.info, "n_ctx", 0) or 0)
@@ -445,18 +458,20 @@ class NativeInferenceService:
             out["repeat_last_n"] = 64
         return out
 
-    @staticmethod
-    def _format(request: InferenceRequest) -> Dict[str, Any]:
+    def _format(self, request: InferenceRequest) -> Dict[str, Any]:
         """The request's output format -> the engine's `format` keyword.  metadata.format first (the gateway's Ollama routes,
         server/src/routes/ollama.ts:229, 385), then options.format (its OpenAI route, openai.ts:636-642).  "json" turns the
-        JSON grammar mask on; so does a JSON-schema object, but the schema itself is NOT enforced (the response is valid JSON of
-        any shape).  Absent, None or "" is free text ({}); anything else fails the request, as a bad temperature does."""
+        JSON grammar mask on.  A JSON-schema object is enforced with json_schema=True (the engine compiles it; see
+        gl_format_schema); otherwise it too turns on the JSON mask alone (valid JSON of any shape).  Absent, None or "" is free
+        text ({}); anything else fails the request, as a bad temperature does."""
         md = request.get("metadata") or {}
         fmt = md.get("format")
         if fmt is None or fmt == "":
             fmt = (request.get("options") or {}).get("format")
         if fmt is None or fmt == "":
             return {}
+        if isinstance(fmt, dict) and self._json_schema:
+            return {"format": fmt}
         if fmt == "json" or isinstance(fmt, dict):
             return {"format": "json"}
         raise RuntimeError(f'format must be "json" or a JSON schema object, not {fmt!r}')

@@ -98,8 +98,8 @@ void read_penalty_opts(napi_env env, napi_value o, gl_sample_opts& so) {
     if (napi_get_named_property(env, o, "presencePenalty", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.presence_penalty = (float)d;
     if (napi_get_named_property(env, o, "frequencyPenalty", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.frequency_penalty = (float)d;
     if (napi_get_named_property(env, o, "minP", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.min_p = (float)d;
-    // output format: "json" (or GL_FORMAT_JSON) turns the JSON grammar mask on; absent, "" or 0 is free text; anything else
-    // reaches the library as it is and is refused there (GL_ERR_INVALID)
+    // output format: "json" (or GL_FORMAT_JSON) turns the JSON grammar mask on, a formatSchema code the schema mask; absent, ""
+    // or 0 is free text; anything else reaches the library as it is and is refused there (GL_ERR_INVALID)
     napi_valuetype vt;
     if (napi_get_named_property(env, o, "format", &v) == napi_ok && napi_typeof(env, v, &vt) == napi_ok) {
         if (vt == napi_string) {
@@ -396,6 +396,24 @@ napi_value TokenText(napi_env env, napi_callback_info info) {
     return out;
 }
 
+// formatSchema(engine, schemaText) -> the gl_format_schema code for a request's `format` (throws with the library's message,
+// e.g. "format schema: 'pattern' is not supported at /properties/zip")
+napi_value FormatSchema(napi_env env, napi_callback_info info) {
+    size_t argc = 2;
+    napi_value argv[2];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    gl_engine* e = unwrap(env, argv[0]);
+    size_t len = 0;
+    NAPI_OK(napi_get_value_string_utf8(env, argv[1], nullptr, 0, &len));
+    std::string text(len + 1, '\0');
+    NAPI_OK(napi_get_value_string_utf8(env, argv[1], &text[0], len + 1, &len));
+    int32_t code = 0;
+    if (gl_format_schema(e, text.data(), (int32_t)len, &code) != GL_OK) return throw_gl(env, "gl_format_schema");
+    napi_value out;
+    NAPI_OK(napi_create_int32(env, code, &out));
+    return out;
+}
+
 void read_sample_opts(napi_env env, napi_value o, gl_sample_opts& so, std::vector<int32_t>& stop_ids) {
     napi_value v;
     so.num_predict = 128;
@@ -570,6 +588,7 @@ napi_value Init(napi_env env, napi_value exports) {
         {"embed", nullptr, Embed, nullptr, nullptr, nullptr, napi_default, nullptr},
         {"chatTemplate", nullptr, ChatTemplate, nullptr, nullptr, nullptr, napi_default, nullptr},
         {"tokenText", nullptr, TokenText, nullptr, nullptr, nullptr, napi_default, nullptr},
+        {"formatSchema", nullptr, FormatSchema, nullptr, nullptr, nullptr, napi_default, nullptr},
         {"seqOpen", nullptr, SeqOpen, nullptr, nullptr, nullptr, napi_default, nullptr},
         {"batchStep", nullptr, BatchStep, nullptr, nullptr, nullptr, napi_default, nullptr},
         {"seqClose", nullptr, SeqClose, nullptr, nullptr, nullptr, napi_default, nullptr},

@@ -29,9 +29,13 @@ export class NativeInferenceService {
 	// prefixCache: a generate keeps the KV pages of the longest prefix it shares with the previous generate on the same engine
 	// (a client that sends `context` back pays for its new tokens only); off by default (include/gridllm_native.h)
 	private engineOptions: { prefixCache?: boolean };
+	// jsonSchema: enforce a JSON-schema `format` on the GPU (gl_format_schema); off by default: a schema asks for valid JSON of
+	// any shape, as before.  Same switch as gridllm_b200/service.py's json_schema.
+	private jsonSchema: boolean;
 
-	constructor(options: { prefixCache?: boolean } = {}) {
+	constructor(options: { prefixCache?: boolean; jsonSchema?: boolean } = {}) {
 		this.engineOptions = { prefixCache: !!options.prefixCache };
+		this.jsonSchema = !!options.jsonSchema;
 	}
 
 	private engine(name: string): unknown {
@@ -159,18 +163,26 @@ export class NativeInferenceService {
 		if (nCtx > 0 && nPrompt < nCtx) numPredict = Math.min(numPredict, nCtx - nPrompt);
 		return { numPredict, ignoreEos: !!o.ignore_eos, temperature, topK: o.top_k ?? d.top_k ?? 0, topP: o.top_p ?? d.top_p ?? 1,
 			seed: BigInt(o.seed ?? (temperature > 0 ? Math.floor(Math.random() * 2 ** 53) : 0)), ...this.penaltyOpts(o),
-			...this.formatOpts(request) };
+			...this.formatOpts(request, e) };
 	}
 
 	// The output format -> the addon's format field; same mapping as gridllm_b200/service.py::_format.  metadata.format first (the
-	// gateway's Ollama routes), then options.format (its OpenAI route).  "json" turns the JSON grammar mask on; so does a JSON-schema
-	// object, whose schema is NOT enforced (the response is valid JSON of any shape).  Absent, null or "": free text.
-	private formatOpts(request: InferenceRequest): { format?: string } {
+	// gateway's Ollama routes), then options.format (its OpenAI route).  "json" turns the JSON grammar mask on.  A JSON-schema
+	// object is compiled and enforced with jsonSchema (a schema outside the subset fails the request with the library's message);
+	// otherwise it too turns on the JSON mask alone (valid JSON of any shape).  Absent, null or "": free text.
+	private formatOpts(request: InferenceRequest, e?: unknown): { format?: string | number } {
 		let f: any = request.metadata?.format;
 		if (f === undefined || f === null || f === "") f = (request.options as Record<string, any> | undefined)?.format;
 		if (f === undefined || f === null || f === "") return {};
 		if (f !== "json" && (typeof f !== "object" || Array.isArray(f))) throw new Error(`format must be "json" or a JSON schema object`);
 		if (request.options?.ignore_eos) throw new Error("format json cannot be combined with ignore_eos: a JSON document ends on a stop token");
+		if (this.jsonSchema && typeof f === "object" && e) {
+			try {
+				return { format: native.formatSchema(e, JSON.stringify(f)) as number };
+			} catch (err: any) {
+				throw new Error(String(err?.message ?? err).replace(/^gl_format_schema: (GL_ERR_[A-Z]+: )?/, ""));
+			}
+		}
 		return { format: "json" };
 	}
 

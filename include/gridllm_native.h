@@ -138,8 +138,8 @@ typedef struct gl_sample_opts {
      * Refused: with ignore_eos (GL_ERR_INVALID); stop_ids that are not control tokens (GL_ERR_INVALID); a model without a
      * tokenizer, or whose vocabulary lacks a single-byte token for each of \t, \n, 0x20-0x7E (and 0x80-0xBF when some piece
      * is not whole well-formed UTF-8), or has no eos (GL_ERR_UNSUPPORTED, checked once, at the first JSON request); gl_generate
-     * on the persistent decode kernel (GL_MEGA=1, GL_ERR_UNSUPPORTED).  JSON schemas are not enforced here: a host maps a
-     * schema to GL_FORMAT_JSON and gets valid JSON of any shape. */
+     * on the persistent decode kernel (GL_MEGA=1, GL_ERR_UNSUPPORTED).  A code >= GL_FORMAT_SCHEMA_BASE from gl_format_schema
+     * holds the bytes to the documents of that JSON schema instead (see there); everything else above applies to it as well. */
     union {
         int32_t  format;
         int32_t  reserved[1];
@@ -147,6 +147,7 @@ typedef struct gl_sample_opts {
 } gl_sample_opts;
 
 #define GL_FORMAT_JSON 1
+#define GL_FORMAT_SCHEMA_BASE 256
 
 typedef struct gl_gen_stats {
     int32_t prompt_eval_count;     /* InferenceResponse.prompt_eval_count (client/src/types/index.ts:61) */
@@ -260,6 +261,38 @@ int  gl_penalize_logits(gl_engine* e, float* logits, int32_t n_vocab, const gl_s
  * Rewinds the sequence like gl_kv_reset(). */
 int  gl_constrain_logits(gl_engine* e, float* logits, int32_t n_vocab, const gl_sample_opts* opts, const int32_t* generated,
                          int32_t n_generated);
+
+/* gl_format_schema: compile a JSON schema (Ollama's `format` as an object) and register it with the engine; *format_out gets
+ * a code >= GL_FORMAT_SCHEMA_BASE for gl_sample_opts.format.  Identical bytes give the same code.  The engine keeps at most
+ * 64 compiled schemas: when full, it evicts the least recently used one that no open sequence uses (GL_ERR_NOMEM when every
+ * one is in use).  Codes are never reused; an unknown or evicted code is GL_ERR_INVALID wherever a format is taken.
+ * Malformed JSON is GL_ERR_INVALID; a schema outside the subset below is GL_ERR_UNSUPPORTED, with a message that names the
+ * keyword and its JSON pointer ("'pattern' is not supported at /properties/zip").
+ * A registered schema S restricts the generated bytes to the documents of S, written with the ws rule, the nesting bound (64,
+ * root included) and the string / number syntax of the GL_FORMAT_JSON language, and:
+ *   - root: an object schema (type "object", properties, or a $ref to one); any other root is refused.
+ *   - objects with properties are closed (additionalProperties absent or false).  Keys come in this order: the required
+ *     properties in `properties` order, then any subset of the optional ones, in `properties` order (llama.cpp's
+ *     json-schema-to-grammar order; unpinned against a real Ollama).  {"type": "object"} without properties is any object.
+ *     Refused: additionalProperties true or a schema, a `required` name that is not in `properties`.
+ *   - arrays: items (absent: any value), minItems, maxItems.  strings: minLength, maxLength, in code points, an escape counting
+ *     as one (so a surrogate pair written as two \u escapes counts as two).  integer: -? (0 | [1-9][0-9]*), no fraction or
+ *     exponent.  number, boolean, null; type lists.
+ *   - enum / const: strings, integers, booleans, null, spelled canonically: compact, UTF-8 as is, only ", \ and U+0000-U+001F
+ *     escaped (\b \f \n \r \t, else \u00xx in lowercase hex) -- Python's json.dumps(ensure_ascii=False).  Keys likewise.
+ *   - anyOf / oneOf: only alternatives whose sets of first value bytes are disjoint (X | null, string | integer, ...).  allOf
+ *     with one member is that member.  $ref: "#", "#/$defs/..", "#/definitions/..", recursion allowed.
+ *   - ignored: title, description, $schema, $id, $comment, examples, default, deprecated, readOnly, writeOnly, discriminator.
+ *     Every other keyword is refused (pattern, format, minimum / maximum / exclusive*, multipleOf, uniqueItems, prefixItems,
+ *     patternProperties, not, if / then / else, ...).
+ *   - no dead ends: a schema whose smallest document nests deeper than 64, an empty enum and min > max are refused; the mask
+ *     never opens a container, picks an optional key or starts an array item from which no document closes within the bound.
+ *   - limits: <= 4 096 nodes, <= 255 properties per object, counts <= 65 534.
+ *   - the vocabulary must have a single-byte token for every byte of the keys and enum members (beside the GL_FORMAT_JSON
+ *     requirements), else GL_ERR_UNSUPPORTED.
+ * Stop tokens, control tokens, penalties before the mask, the first draw after the prompt, logprobs and gl_*_logits are as for
+ * GL_FORMAT_JSON; gl_constrain_logits takes schema codes.  Refused under GL_MEGA=1. */
+int  gl_format_schema(gl_engine* e, const char* schema_utf8, int32_t n_bytes, int32_t* format_out);
 
 /* ---- kernel-level entry points (parity tests and roofline measurement) ------------------ */
 /* y[rows] = W[rows x cols] (GGUF-layout blocks of ggml_type, host memory) * x[cols].
