@@ -29,10 +29,8 @@ struct StepState {
     int pen_last_n;     // window: > 0 the last N history ids, -1 the whole history
     float repeat_penalty;     // 1 = off
     float presence_penalty, frequency_penalty;
-    // JSON grammar mask (json_mask.cu); json = 0: none.  json_st[i & 1]: the automaton state (json_fsm.h JsonState, 16 bytes)
-    // after the output's first i tokens -- written by the mask kernel of output i, read by that of output i + 1
+    // 1: the JSON grammar mask runs on this sequence (schema_mask.cu; its automaton state lives in its SchemaSlot); 0: none
     int json;
-    unsigned json_st[2][4];
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }

@@ -434,7 +434,14 @@ Status Engine::ensure_pages(int n_tokens) {
     return {};
 }
 
-StepState Engine::make_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so, int* sampler, int* penalised) const {
+// repetition penalties (penalty.cu): repeat_penalty is active when > 0 and != 1; a window of 0, or nothing active, is no penalty
+// at all, and such a request replays exactly the graphs of a request without the fields
+static bool repeat_penalty_on(const gl_sample_opts& so) { return so.repeat_penalty > 0.f && so.repeat_penalty != 1.f; }
+static bool penalties_on(const gl_sample_opts& so) {
+    return so.repeat_last_n != 0 && (repeat_penalty_on(so) || so.presence_penalty != 0.f || so.frequency_penalty != 0.f);
+}
+
+StepState Engine::make_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so) const {
     StepState h{};
     h.pos = pos; h.token = token; h.n_prompt = n_prompt; h.out_idx = out_idx; h.done = 0;
     h.ignore_eos = so ? so->ignore_eos : 1;
@@ -445,33 +452,55 @@ StepState Engine::make_state(int pos, int token, int n_prompt, int out_idx, cons
         for (int i = 0; i < so->n_stop_ids && h.n_stop < 8; ++i) h.stop_ids[h.n_stop++] = so->stop_ids[i];
     }
     h.bar_base = 0;
-    // 0 greedy; 1 two-stage top-k sampler (top_k <= 64); 2 single-CTA radix select (sampler.cu)
-    if (sampler) *sampler = !(so && so->temperature > 0.f) ? 0 : (sample_topk_fast_applies(so->top_k, n_vocab_) ? 1 : 2);
     h.temperature = so ? so->temperature : 0.f;
     h.top_k = so ? so->top_k : 0;
     h.top_p = (so && so->top_p > 0.f) ? so->top_p : 1.f;
     h.seed_lo = so ? (unsigned)(so->seed & 0xffffffffull) : 0u;
     h.seed_hi = so ? (unsigned)(so->seed >> 32) : 0u;
     h.min_p = (so && so->min_p > 0.f) ? so->min_p : 0.f;
-    // repetition penalties (penalty.cu): repeat_penalty is active when > 0 and != 1; a window of 0, or nothing active, is no
-    // penalty at all, and such a request replays exactly the graphs of a request without the fields
-    const bool rp_on = so && so->repeat_penalty > 0.f && so->repeat_penalty != 1.f;
-    const bool pen = so && so->repeat_last_n != 0 && (rp_on || so->presence_penalty != 0.f || so->frequency_penalty != 0.f);
+    const bool pen = so && penalties_on(*so);
     h.pen_last_n = pen ? so->repeat_last_n : 0;
-    h.repeat_penalty = rp_on ? so->repeat_penalty : 1.f;
+    h.repeat_penalty = so && repeat_penalty_on(*so) ? so->repeat_penalty : 1.f;
     h.presence_penalty = pen ? so->presence_penalty : 0.f;
     h.frequency_penalty = pen ? so->frequency_penalty : 0.f;
-    if (penalised) *penalised = pen ? 1 : 0;
-    // JSON grammar mask (json_mask.cu): json_st starts zeroed, the automaton's initial state; 2: a registered schema
-    // (schema_mask.cu), whose state lives in the sequence's SchemaSlot
-    h.json = !so ? 0 : so->format == GL_FORMAT_JSON ? 1 : so->format >= GL_FORMAT_SCHEMA_BASE ? 2 : 0;
+    h.json = so && so->format ? 1 : 0;          // the grammar mask's state lives in the sequence's SchemaSlot
     return h;
 }
 
-Status Engine::set_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so) {
-    const StepState h = make_state(pos, token, n_prompt, out_idx, so, &sampler_, &penalised_);
-    json_ = h.json;
-    if (h.json == 2) ST(schema_bind(schema_entry(), so->format));
+Status Engine::plan_draw(const gl_sample_opts& so, bool single_path, DrawPlan* plan) {
+    if (!(so.temperature >= 0.f) || !std::isfinite(so.temperature)) return fail(GL_ERR_INVALID, "temperature must be a finite number >= 0");
+    DrawPlan d;
+    // 0 greedy; 1 two-stage top-k sampler (top_k <= 64); 2 single-CTA radix select (sampler.cu)
+    d.sampler = so.temperature > 0.f ? (sample_topk_fast_applies(so.top_k, n_vocab_) ? 1 : 2) : 0;
+    d.penalised = penalties_on(so);
+    d.masked = so.format != 0;
+    d.format = so.format;
+    const bool mega = single_path && use_mega_;
+    if (mega && d.sampler) return fail(GL_ERR_UNSUPPORTED, "the persistent decode kernel (GL_MEGA=1) samples greedily only");
+    if (mega && d.penalised) return fail(GL_ERR_UNSUPPORTED, "the persistent decode kernel (GL_MEGA=1) has no repetition penalties");
+    if (d.masked) {
+        // the value range of format and its clash with ignore_eos are checked at the C boundary (c_api.cpp check_format)
+        const bool schema = so.format >= GL_FORMAT_SCHEMA_BASE;
+        if (schema && !schemas_.count(so.format)) return fail(GL_ERR_INVALID, "format: unknown or evicted schema code " + std::to_string(so.format));
+        if (mega) return fail(GL_ERR_UNSUPPORTED, "the persistent decode kernel (GL_MEGA=1) has no JSON grammar mask");
+        ST(ensure_json());
+        ST(ensure_schema_state());
+        if (schema) schemas_[so.format].used = ++schema_clock_;
+        // a stop id that is an ordinary token would be masked wherever it is needed, and the vocabulary guarantee would not hold
+        for (int i = 0; i < so.n_stop_ids; ++i) {
+            const int32_t id = so.stop_ids ? so.stop_ids[i] : -1;
+            if (id >= 0 && id < n_vocab_ && json_hoff_[id + 1] != json_hoff_[id])
+                return fail(GL_ERR_INVALID, "format json: stop_ids must be control tokens (empty piece); use stop strings for text");
+        }
+    }
+    *plan = d;
+    return {};
+}
+
+Status Engine::set_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so, const DrawPlan& plan) {
+    const StepState h = make_state(pos, token, n_prompt, out_idx, so);
+    plan_ = plan;
+    if (plan.masked) ST(schema_bind(schema_entry(), plan.format));
     if (bar_counter_) CU(cudaMemsetAsync(bar_counter_, 0, 4, stream_));
     CU(cudaMemcpyAsync(st_, &h, sizeof(h), cudaMemcpyHostToDevice, stream_));
     CU(cudaStreamSynchronize(stream_));     // h is on the stack
@@ -627,25 +656,35 @@ Status Engine::enqueue_head(cudaStream_t s, bool keep_logits, int* n_launch) {
         CU(rmsnorm_launch(x_, output_norm_, n_embd_, eps_, xn_, s)); ++*n_launch;
         ST(plain_gemv(s, output_, xn_, logits_, n_launch));
     }
-    if (penalised_) {          // repetition penalties on the logits before the draw (penalty.cu); plain stream order after the lm_head
-        PenaltyParams pp{logits_, n_vocab_, st_, nullptr, prompt_ids_, 0, out_ids_, 0, pen_counts_};
-        CU(penalty_launch(pp, 1, false, s));
-        ++*n_launch;
-    }
-    if (json_ == 2) {          // a JSON schema: the schema mask in the JSON mask's place (schema_mask.cu)
-        SchemaMaskParams sp{logits_, n_vocab_, st_, nullptr, schema_entry(), json_tab_, json_off_, json_bytes_, json_cls_};
-        CU(schema_mask_launch(sp, 1, false, s));
-        ++*n_launch;
-    } else if (json_) {        // the JSON grammar mask after the penalties, right before the draw (json_mask.cu)
-        JsonMaskParams jp{logits_, n_vocab_, st_, nullptr, json_off_, json_bytes_, json_cls_};
-        CU(json_mask_launch(jp, 1, false, s));
-        ++*n_launch;
-    }
+    CU(enqueue_pre_draw(s, 0, plan_.penalised, plan_.masked, prompt_ids_, n_launch));
     SampleParams sp{logits_, n_vocab_, st_, out_ids_, out_lp_, keep_logits ? logits_keep_ : nullptr, keep_logits ? keep_cap_ : max_out_, sample_scratch_, topk_scratch_};
-    if (sampler_ != 0) CU(sample_topk_launch(sp, sampler_ == 1, pdl && fused_ && sampler_pdl_, s));      // temperature > 0: seeded top-k / top-p draw (sampler.cu)
+    if (plan_.sampler != 0) CU(sample_topk_launch(sp, plan_.sampler == 1, pdl && fused_ && sampler_pdl_, s));      // temperature > 0: seeded top-k / top-p draw (sampler.cu)
     else CU(sample_greedy_launch(sp, pdl && fused_ && greedy_pdl_, s));
     ++*n_launch;
     return {};
+}
+
+// The penalty and mask kernels launch without programmatic dependent launch: plain stream order after the lm_head.
+cudaError_t Engine::enqueue_pre_draw(cudaStream_t s, int bucket, bool penalised, bool masked, const int* prompt, int* n_launch) {
+    const bool one = bucket == 0;
+    float* logits = one ? logits_ : blogits_;
+    StepState* st = one ? st_ : bst_;
+    const BatchCtl* ctl = one ? nullptr : bctl_;
+    const int rows = one ? 1 : bucket;
+    if (penalised) {
+        const PenaltyParams pp = one ? PenaltyParams{logits, n_vocab_, st, ctl, prompt, 0, out_ids_, 0, pen_counts_}
+                                     : PenaltyParams{logits, n_vocab_, st, ctl, bprompt_, n_ctx_, bout_ids_, max_out_, bpen_counts_};
+        const cudaError_t e = penalty_launch(pp, rows, false, s);
+        if (e != cudaSuccess) return e;
+        if (n_launch) ++*n_launch;
+    }
+    if (masked) {
+        const SchemaMaskParams mp{logits, n_vocab_, st, ctl, one ? schema_entry() : sch_ + 1, json_off_, json_bytes_, json_cls_};
+        const cudaError_t e = schema_mask_launch(mp, rows, false, s);
+        if (e != cudaSuccess) return e;
+        if (n_launch) ++*n_launch;
+    }
+    return cudaSuccess;
 }
 
 Status Engine::build_graphs() {
@@ -673,9 +712,9 @@ Status Engine::run_steps(int n_nohead, int n_head, bool keep_logits) {
         if (n_head > 0) ST(launch_mega(n_head, true, keep_logits));
         return {};
     }
-    // the step with a head exists in 36 captured variants (sampler x plain / logits kept x without / with the penalty kernel x
-    // without format / with the JSON mask kernel / with the schema mask kernel); all but the first lazily
-    cudaGraphExec_t* head = &g_head_var_[sampler_][keep_logits ? 1 : 0][penalised_ ? 1 : 0][json_];
+    // the step with a head exists in 24 captured variants (sampler x plain / logits kept x without / with the penalty kernel x
+    // without / with the mask kernel); all but the first lazily
+    cudaGraphExec_t* head = &g_head_var_[plan_.sampler][keep_logits ? 1 : 0][plan_.penalised ? 1 : 0][plan_.masked ? 1 : 0];
     if (use_graph_ && n_head > 0 && !*head) {
         cudaGraph_t g = nullptr;
         CU(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
@@ -817,14 +856,8 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
     const int64_t t0 = now_ns();
     if (n_prompt <= 0 || !prompt) return fail(GL_ERR_INVALID, "empty prompt");
     const int n_pred = so.num_predict > 0 ? so.num_predict : 128;     // OllamaService.ts:105
-    if (!(so.temperature >= 0.f) || !std::isfinite(so.temperature)) return fail(GL_ERR_INVALID, "temperature must be a finite number >= 0");
-    if (so.temperature > 0.f && use_mega_) return fail(GL_ERR_UNSUPPORTED, "the persistent decode kernel (GL_MEGA=1) samples greedily only");
-    if (use_mega_) {
-        int pen = 0;
-        make_state(0, 0, n_prompt, 0, &so, nullptr, &pen);
-        if (pen) return fail(GL_ERR_UNSUPPORTED, "the persistent decode kernel (GL_MEGA=1) has no repetition penalties");
-    }
-    ST(json_admit(so, true));
+    DrawPlan plan;
+    ST(plan_draw(so, true, &plan));
     for (int i = 0; i < n_prompt; ++i)
         if (prompt[i] < 0 || prompt[i] >= n_vocab_) return fail(GL_ERR_INVALID, "prompt token id out of range");
     // prefix reuse: keep the pages of the positions the previous request left final and that this prompt repeats
@@ -856,13 +889,13 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
     const int mega0 = mega_launches_;
     if (batched) {
         // prompt positions [reuse, n_prompt) through the tensor-core path; the sampler then moves pos from T-1 to T
-        ST(set_state(n_prompt - 1, prompt[n_prompt - 1], n_prompt, 0, &so));
+        ST(set_state(n_prompt - 1, prompt[n_prompt - 1], n_prompt, 0, &so, plan));
         CU(cudaEventRecord(ev_[0], stream_));
         ST(prefill_batched(reuse, n_prompt - reuse, &prefill_launches));
         CU(cudaEventRecord(ev_[1], stream_));
     } else {
         // sequential prefill: positions reuse .. n_prompt-2 without a head, then the last prompt token produces token 0
-        ST(set_state(reuse, prompt[reuse], n_prompt, 0, &so));
+        ST(set_state(reuse, prompt[reuse], n_prompt, 0, &so, plan));
         CU(cudaEventRecord(ev_[0], stream_));
         ST(run_steps(n_prompt - 1 - reuse, 0, false));
         CU(cudaEventRecord(ev_[1], stream_));
@@ -944,14 +977,16 @@ Status Engine::sample_logits(const float* logits, int n_vocab, const gl_sample_o
     CU(cudaSetDevice(device_));
     if (!logits || n_vocab != n_vocab_) return fail(GL_ERR_INVALID, "logits must hold n_vocab values");
     if (out_index < 0 || out_index >= max_out_) return fail(GL_ERR_INVALID, "output index out of range");
-    if (!(so.temperature >= 0.f) || !std::isfinite(so.temperature)) return fail(GL_ERR_INVALID, "temperature must be a finite number >= 0");
-    ST(kv_reset());
     gl_sample_opts o = so;
     o.ignore_eos = 1;
-    ST(set_state(0, 0, 0, out_index, &o));
+    o.format = 0;                                      // the sampler alone: the format is not looked at
+    DrawPlan plan;
+    ST(plan_draw(o, false, &plan));
+    ST(kv_reset());
+    ST(set_state(0, 0, 0, out_index, &o, plan));
     CU(cudaMemcpyAsync(logits_, logits, (size_t)n_vocab_ * 4, cudaMemcpyHostToDevice, stream_));
     SampleParams sp{logits_, n_vocab_, st_, out_ids_, out_lp_, nullptr, max_out_, sample_scratch_, topk_scratch_};
-    if (sampler_ != 0) CU(sample_topk_launch(sp, sampler_ == 1, false, stream_));
+    if (plan.sampler != 0) CU(sample_topk_launch(sp, plan.sampler == 1, false, stream_));
     else CU(sample_greedy_launch(sp, false, stream_));
     int tid = 0;
     float lp = 0.f;
@@ -972,20 +1007,21 @@ Status Engine::penalize_logits(float* logits, int n_vocab, const gl_sample_opts&
     if (n_history < 0 || (n_history > 0 && !history)) return fail(GL_ERR_INVALID, "bad history");
     for (int i = 0; i < n_history; ++i)
         if (history[i] < 0 || history[i] >= n_vocab_) return fail(GL_ERR_INVALID, "history token id out of range");
-    ST(kv_reset());
     gl_sample_opts o = so;
     o.ignore_eos = 1;
-    ST(set_state(0, 0, n_history, 0, &o));
+    o.temperature = 0.f;                               // the penalty kernel alone: no draw and no mask
+    o.format = 0;
+    DrawPlan plan;
+    ST(plan_draw(o, false, &plan));
+    ST(kv_reset());
+    ST(set_state(0, 0, n_history, 0, &o, plan));
     int* hist = nullptr;
     if (n_history > 0) CU(cudaMalloc((void**)&hist, (size_t)n_history * 4));
     Status rs;
     do {
         cudaError_t ce = hist ? cudaMemcpyAsync(hist, history, (size_t)n_history * 4, cudaMemcpyHostToDevice, stream_) : cudaSuccess;
         if (ce == cudaSuccess) ce = cudaMemcpyAsync(logits_, logits, (size_t)n_vocab_ * 4, cudaMemcpyHostToDevice, stream_);
-        if (ce == cudaSuccess && penalised_ && hist) {
-            PenaltyParams pp{logits_, n_vocab_, st_, nullptr, hist, 0, out_ids_, 0, pen_counts_};
-            ce = penalty_launch(pp, 1, false, stream_);
-        }
+        if (ce == cudaSuccess && hist) ce = enqueue_pre_draw(stream_, 0, plan.penalised, false, hist);
         if (ce == cudaSuccess) ce = cudaMemcpyAsync(logits, logits_, (size_t)n_vocab_ * 4, cudaMemcpyDeviceToHost, stream_);
         if (ce == cudaSuccess) ce = cudaStreamSynchronize(stream_);
         if (ce != cudaSuccess) rs = fail(GL_ERR_CUDA, std::string("penalize_logits: ") + cudaGetErrorString(ce));
@@ -995,7 +1031,7 @@ Status Engine::penalize_logits(float* logits, int n_vocab, const gl_sample_opts&
     return kv_reset();
 }
 
-// ---- JSON grammar mask (json_mask.cu) --------------------------------------------------------------------------------
+// ---- JSON grammar mask (schema_mask.cu) ------------------------------------------------------------------------------
 // The vocabulary table the mask kernel reads, built once at the first JSON request.  The vocabulary must guarantee that every
 // state the automaton can reach has an allowed token, so that the mask never leaves a draw with nothing: a single-byte piece for
 // each of \t, \n and 0x20-0x7E (all of them ordinary tokens, not stop tokens), one for each of 0x80-0xBF as soon as some piece
@@ -1063,31 +1099,10 @@ Status Engine::ensure_json() {
 }
 
 bool Engine::json_stop(const gl_sample_opts& so, int32_t id) const {
-    const StepState h = make_state(0, 0, 0, 0, &so, nullptr);      // the stop ids the device sees
+    const StepState h = make_state(0, 0, 0, 0, &so);      // the stop ids the device sees
     for (int k = 0; k < h.n_stop; ++k)
         if (h.stop_ids[k] == id) return true;
     return false;
-}
-
-Status Engine::json_admit(const gl_sample_opts& so, bool single_path) {
-    if (so.format == 0) return {};
-    const bool schema = so.format >= GL_FORMAT_SCHEMA_BASE;
-    if (so.format != GL_FORMAT_JSON && !schema) return fail(GL_ERR_INVALID, "format must be 0 (off), GL_FORMAT_JSON or a gl_format_schema code");
-    if (schema && !schemas_.count(so.format)) return fail(GL_ERR_INVALID, "format: unknown or evicted schema code " + std::to_string(so.format));
-    if (so.ignore_eos) return fail(GL_ERR_INVALID, "format json cannot be combined with ignore_eos: a JSON document ends on a stop token");
-    if (single_path && use_mega_) return fail(GL_ERR_UNSUPPORTED, "the persistent decode kernel (GL_MEGA=1) has no JSON grammar mask");
-    ST(ensure_json());
-    if (schema) {
-        ST(ensure_schema_state());
-        schemas_[so.format].used = ++schema_clock_;
-    }
-    // a stop id that is an ordinary token would be masked wherever it is needed, and the vocabulary guarantee would not hold
-    for (int i = 0; i < so.n_stop_ids; ++i) {
-        const int32_t id = so.stop_ids ? so.stop_ids[i] : -1;
-        if (id >= 0 && id < n_vocab_ && json_hoff_[id + 1] != json_hoff_[id])
-            return fail(GL_ERR_INVALID, "format json: stop_ids must be control tokens (empty piece); use stop strings for text");
-    }
-    return {};
 }
 
 // The automaton through a caller-supplied output history, then the mask kernel alone on caller-supplied logits (parity tests
@@ -1101,45 +1116,33 @@ Status Engine::constrain_logits(float* logits, int n_vocab, const gl_sample_opts
         if (generated[i] < 0 || generated[i] >= n_vocab_) return fail(GL_ERR_INVALID, "history token id out of range");
     gl_sample_opts o = so;
     o.ignore_eos = 0;
+    o.temperature = 0.f;                               // the mask alone: no draw
     if (o.format == 0) return {};                      // off: the logits stay as they are
-    ST(json_admit(o, false));
+    DrawPlan plan;
+    ST(plan_draw(o, false, &plan));
     // the history must be a prefix the mask allows: no stop token (it would have ended the output), no control token, every
     // byte accepted
-    const bool schema = o.format >= GL_FORMAT_SCHEMA_BASE;
-    JsonState hs{};
     SchemaState ss;
-    SchemaView sv{};
     SchemaArrayFrames sf{ss.fr};
-    if (schema) {
-        sv = schema_view(schemas_[o.format].blob.data());
-        schema_init(ss.js, ss.cur, sv);
-    }
+    const SchemaView sv = schema_view(o.format == GL_FORMAT_JSON ? json_blob_.data() : schemas_[o.format].blob.data());
+    schema_init(ss.js, ss.cur, sv);
     for (int i = 0; i < n_generated; ++i) {
         const int32_t t = generated[i];
         const uint32_t a = json_hoff_[t], b = json_hoff_[t + 1];
-        const bool ok = schema ? schema_run(sv, ss.js, ss.cur, sf, json_hbytes_.data() + a, (int)(b - a))
-                               : json_run(hs, json_hbytes_.data() + a, (int)(b - a));
+        const bool ok = schema_run(sv, ss.js, ss.cur, sf, json_hbytes_.data() + a, (int)(b - a));
         if (json_stop(o, t) || a == b || !ok)
             return fail(GL_ERR_INVALID, "format json: the history is not a prefix the grammar allows (token " + std::to_string(i) + ")");
     }
     ST(kv_reset());
-    ST(set_state(0, n_generated > 0 ? generated[n_generated - 1] : 0, 0, n_generated, &o));
+    ST(set_state(0, n_generated > 0 ? generated[n_generated - 1] : 0, 0, n_generated, &o, plan));
     int* hist = nullptr;
     if (n_generated > 0) CU(cudaMalloc((void**)&hist, (size_t)n_generated * 4));
     Status rs;
     do {
         cudaError_t ce = hist ? cudaMemcpyAsync(hist, generated, (size_t)n_generated * 4, cudaMemcpyHostToDevice, stream_) : cudaSuccess;
-        if (ce == cudaSuccess && hist)
-            ce = schema ? schema_replay_launch(sch_, hist, n_generated, json_off_, json_bytes_, stream_)
-                        : json_replay_launch(st_, hist, n_generated, json_off_, json_bytes_, stream_);
+        if (ce == cudaSuccess && hist) ce = schema_replay_launch(sch_, hist, n_generated, json_off_, json_bytes_, stream_);
         if (ce == cudaSuccess) ce = cudaMemcpyAsync(logits_, logits, (size_t)n_vocab_ * 4, cudaMemcpyHostToDevice, stream_);
-        if (ce == cudaSuccess && schema) {
-            SchemaMaskParams sp{logits_, n_vocab_, st_, nullptr, sch_, json_tab_, json_off_, json_bytes_, json_cls_};
-            ce = schema_mask_launch(sp, 1, false, stream_);
-        } else if (ce == cudaSuccess) {
-            JsonMaskParams jp{logits_, n_vocab_, st_, nullptr, json_off_, json_bytes_, json_cls_};
-            ce = json_mask_launch(jp, 1, false, stream_);
-        }
+        if (ce == cudaSuccess) ce = enqueue_pre_draw(stream_, 0, false, true);
         if (ce == cudaSuccess) ce = cudaMemcpyAsync(logits, logits_, (size_t)n_vocab_ * 4, cudaMemcpyDeviceToHost, stream_);
         if (ce == cudaSuccess) ce = cudaStreamSynchronize(stream_);
         if (ce != cudaSuccess) rs = fail(GL_ERR_CUDA, std::string("constrain_logits: ") + cudaGetErrorString(ce));
@@ -1167,6 +1170,7 @@ Status Engine::ensure_schema_state() {
     CU(cudaMemcpy(t, blob.data(), blob.size(), cudaMemcpyHostToDevice));
     sch_ = d;
     json_tab_ = t;
+    json_blob_ = std::move(blob);
     return {};
 }
 
@@ -1174,10 +1178,14 @@ SchemaSlot* Engine::schema_entry() const {
     return (bst_ && st_ >= bst_ && st_ < bst_ + MAX_BATCH) ? sch_ + 1 + (st_ - bst_) : sch_;
 }
 
-Status Engine::schema_bind(SchemaSlot* e, int code) {
-    auto it = schemas_.find(code);
-    if (it == schemas_.end() || !e) return fail(GL_ERR_INVALID, "format: unknown or evicted schema code " + std::to_string(code));
-    CU(cudaMemcpyAsync(&e->tab, &it->second.dev, sizeof(it->second.dev), cudaMemcpyHostToDevice, stream_));
+Status Engine::schema_bind(SchemaSlot* e, int format) {
+    const uint8_t* const* tab = &json_tab_;
+    if (format != GL_FORMAT_JSON) {
+        auto it = schemas_.find(format);
+        if (it == schemas_.end()) return fail(GL_ERR_INVALID, "format: unknown or evicted schema code " + std::to_string(format));
+        tab = &it->second.dev;
+    }
+    CU(cudaMemcpyAsync(&e->tab, tab, sizeof(*tab), cudaMemcpyHostToDevice, stream_));
     CU(cudaStreamSynchronize(stream_));
     return {};
 }
@@ -1217,7 +1225,7 @@ Status Engine::format_schema(const char* text, int n, int* code) {
         uint64_t oldest = UINT64_MAX;
         for (auto& kv : schemas_) {
             bool in_use = false;
-            for (auto& S : slots_) in_use = in_use || (S.open && S.schema == kv.first);
+            for (auto& S : slots_) in_use = in_use || (S.open && S.plan.format == kv.first);
             if (!in_use && kv.second.used < oldest) { oldest = kv.second.used; victim = kv.first; }
         }
         if (victim < 0) return fail(GL_ERR_NOMEM, "format schema: all 64 registered schemas are in use by open sequences");

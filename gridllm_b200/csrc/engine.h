@@ -48,6 +48,15 @@ struct Status {
     bool ok() const { return code == GL_OK; }
 };
 
+// What runs on a request's logits between the lm_head and its draw (Engine::plan_draw): the penalty kernel, then the grammar
+// mask, then the sampler.
+struct DrawPlan {
+    int sampler = 0;           // 0 greedy (argmax), 1 / 2: the two kernels of sampler.cu (temperature > 0)
+    bool penalised = false;    // repetition penalties that are not a no-op: penalty.cu runs first
+    bool masked = false;       // format json or a schema: schema_mask.cu runs next
+    int format = 0;            // the format the mask follows: GL_FORMAT_JSON or a gl_format_schema code (0: none)
+};
+
 class Engine {
 public:
     static Status create(const std::string& path, int device, const gl_engine_opts* opts, Engine** out);
@@ -95,9 +104,15 @@ private:
     Status enqueue_gemv(cudaStream_t s, GemvParams& p, const GemvMat* mats, int nmat, bool pair, int cols, int* n_launch);
     Status plain_gemv(cudaStream_t s, const DevMatrix& m, const float* x, float* y, int* n_launch);
     Status build_graphs();
-    Status set_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so);
-    // *penalised (optional): 1 when the request's repetition penalties are not a no-op (penalty.cu must run before its draws)
-    StepState make_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so, int* sampler, int* penalised = nullptr) const;
+    // a request's draw: validates what the engine checks of its options (temperature, format, the GL_MEGA=1 refusals when
+    // single_path) and builds the format's tables on first use
+    Status plan_draw(const gl_sample_opts& so, bool single_path, DrawPlan* plan);
+    // the sequence whose step state st_ points at starts over with these options and this plan (its schema bound when masked)
+    Status set_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so, const DrawPlan& plan = DrawPlan{});
+    StepState make_state(int pos, int token, int n_prompt, int out_idx, const gl_sample_opts* so) const;
+    // the kernels between the lm_head and the draw, in order: the penalties, then the grammar mask.  bucket 0: the sequence st_
+    // points at (penalty history: `prompt`, then out_ids_); else the rows of a batched step of that bucket
+    cudaError_t enqueue_pre_draw(cudaStream_t s, int bucket, bool penalised, bool masked, const int* prompt = nullptr, int* n_launch = nullptr);
     Status run_steps(int n_nohead, int n_head, bool keep_logits);
     Status enqueue_head(cudaStream_t s, bool keep_logits, int* n_launch);
     Status build_prefill_weights();
@@ -212,7 +227,8 @@ private:
     struct SeqSlot {
         bool open = false, done = false, first_pending = false;
         std::vector<int> pages;
-        int n_prompt = 0, n_pred = 0, produced = 0, sampler = 0, penalised = 0, json = 0, schema = 0;     // schema: its format code
+        int n_prompt = 0, n_pred = 0, produced = 0;
+        DrawPlan plan;
         int32_t last_token = 0;
         float first_lp = 0.f;
         int last_row = -1;                            // row of the last batched step this sequence took part in
@@ -249,33 +265,26 @@ private:
     std::string qg_why_not_;                          // why the quantised path is unavailable for this model (message for batch_weights = 2)
     Status build_qgemm_weights();
     Status pack_qgemm(const std::vector<const GGUFTensor*>& src, int mode, QGemmWeights& out, uint8_t*& tmp, size_t& tmp_cap);
-    // [bucket][variant]: variant bit 0 the penalty kernel (steps in which some row has penalties), bit 1 the JSON mask kernel
-    // (steps in which some row has format json)
-    // bit 2 the schema mask kernel (steps in which some row has a schema; it also masks the format json rows, so bit 1 is
-    // then clear)
-    cudaGraphExec_t g_batch_[N_BUCKETS][8] = {};
-    int batch_launches_ = 0;                          // kernels of one batched step (without the penalty / JSON mask kernels)
+    // [bucket][variant]: variant bit 0 the penalty kernel (steps in which some row has penalties), bit 1 the grammar mask
+    // kernel (steps in which some row has a format)
+    cudaGraphExec_t g_batch_[N_BUCKETS][4] = {};
+    int batch_launches_ = 0;                          // kernels of one batched step (without the penalty / mask kernels)
     uint64_t bc_[8] = {};                             // gl_batch_counters
     Status ensure_batch_state();
     Status seq_open_single(const int32_t* prompt, int n_prompt, const gl_sample_opts& so, int* slot);
-    Status enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bool json, int* n_launch, bool schema = false);
-    Status run_batch_graph(int bucket, bool penalised, bool json, bool schema = false);
-    cudaError_t batch_schema_launch(int bucket, cudaStream_t s);
-    bool batch_schema_checked_ = false;               // the batched schema mask launch has run once outside stream capture
-    cudaError_t batch_penalty_launch(int bucket, cudaStream_t s);
-    cudaError_t batch_json_launch(int bucket, cudaStream_t s);
-    bool batch_json_checked_ = false;                 // the batched mask launch has run once outside stream capture
+    Status enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bool masked, int* n_launch);
+    Status run_batch_graph(int bucket, bool penalised, bool masked);
+    int batch_checked_ = 0;                           // variant bits whose kernels have run once outside stream capture
+    Status check_pre_draw(int variant);
     Status ensure_batch_penalty();                    // bprompt_ / bpen_counts_, allocated when the first penalised sequence opens
     Status keep_prompt(int slot, const int32_t* prompt, int n_prompt);     // a penalised slot's prompt -> bprompt_
     static int bucket_of(int rows) { int b = 8; while (b < rows) b <<= 1; return b; }
     static int bucket_index(int bucket) { int i = 0; while ((8 << i) < bucket) ++i; return i; }
 
     cudaGraphExec_t g_nohead_ = nullptr;
-    cudaGraphExec_t g_head_var_[3][2][2][3] = {};   // [sampler of the running request][logits kept][repetition penalties][json_]
-    int penalised_ = 0;                        // the running request has penalties: penalty.cu runs between the lm_head and the sampler
-    int json_ = 0;                             // the running request has format json (1: json_mask.cu runs right before the sampler)
-                                               // or a schema (2: schema_mask.cu does)
-    // JSON grammar mask (json_mask.cu): the vocabulary's pieces on the device, built at the first JSON request (nothing before)
+    cudaGraphExec_t g_head_var_[3][2][2][2] = {};   // [sampler][logits kept][penalty kernel][mask kernel] of the running request
+    DrawPlan plan_;                            // the running request's draw
+    // JSON grammar mask (schema_mask.cu): the vocabulary's pieces on the device, built at the first JSON request (nothing before)
     uint32_t* json_off_ = nullptr;             // [n_vocab + 1] byte offsets
     uint8_t* json_bytes_ = nullptr;            // pieces back to back
     uint8_t* json_cls_ = nullptr;              // [n_vocab] JSON_CLS_* bits
@@ -284,8 +293,6 @@ private:
     bool json_checked_ = false;
     std::string json_refused_;                 // why this model cannot take JSON requests ("" once the table is built)
     Status ensure_json();
-    // a request's format field: GL_ERR_UNSUPPORTED / GL_ERR_INVALID when the engine cannot honour it (table built on first use)
-    Status json_admit(const gl_sample_opts& so, bool single_path);
     bool json_stop(const gl_sample_opts& so, int32_t id) const;     // id is a stop token of a request with these options
     // JSON schemas (gl_format_schema; schema_mask.cu): at most SCHEMA_CACHE compiled schemas by code, least recently used
     // evicted first unless an open sequence uses it; codes are never reused
@@ -295,12 +302,13 @@ private:
     std::map<std::string, int> schema_codes_;
     int next_schema_ = GL_FORMAT_SCHEMA_BASE;
     uint64_t schema_clock_ = 0;
-    // per-sequence schema state, allocated at the first schema request: [0] the single-sequence path, [1 + slot] batch slots
+    // per-sequence mask state, allocated at the first JSON request: [0] the single-sequence path, [1 + slot] batch slots
     SchemaSlot* sch_ = nullptr;
-    uint8_t* json_tab_ = nullptr;              // the built-in any-object schema (format json rows in a schema mask launch)
+    uint8_t* json_tab_ = nullptr;              // the built-in any-object schema: what format json rows follow
+    std::vector<uint8_t> json_blob_;           // ... its host copy (history validation of gl_constrain_logits)
     Status ensure_schema_state();
     SchemaSlot* schema_entry() const;          // the entry of the sequence whose step state st_ points at
-    Status schema_bind(SchemaSlot* e, int code);     // e follows schema `code` from its next output 0
+    Status schema_bind(SchemaSlot* e, int format);   // e follows format json or schema `format` from its next output 0
 public:
     Status format_schema(const char* text, int n, int* code);
 private:
@@ -308,9 +316,8 @@ private:
     // beside the lm_head CTAs cost the step 60 us (run 67: 1.537 -> 1.478 ms/token at top_k 40); the greedy sampler keeps it.
     bool sampler_pdl_ = false;
     bool greedy_pdl_ = false;                 // the greedy sampler likewise (64 small CTAs: 3 us per token, run 68)
-    int sampler_ = 0;                          // 0 greedy (argmax), 1 / 2: the two kernels of sampler.cu (temperature > 0)
-    int launches_nohead_ = 0, launches_head_ = 0;    // launches_head_: the step with a head WITHOUT the penalty kernel
-    int head_launches() const { return launches_head_ + (use_mega_ ? 0 : (penalised_ ? 1 : 0) + (json_ ? 1 : 0)); }     // ... of the variant that runs
+    int launches_nohead_ = 0, launches_head_ = 0;    // launches_head_: the step with a head WITHOUT the penalty / mask kernels
+    int head_launches() const { return launches_head_ + (use_mega_ ? 0 : (plan_.penalised ? 1 : 0) + (plan_.masked ? 1 : 0)); }     // ... of the variant that runs
     cudaEvent_t ev_[4] = {nullptr, nullptr, nullptr, nullptr};
     int64_t load_ns_ = 0;
     uint64_t weight_bytes_ = 0, decode_bytes_ = 0, n_params_ = 0;

@@ -198,9 +198,6 @@ Status Engine::ensure_batch_penalty() {
     CU(cudaMemsetAsync(cnt, 0, (size_t)max_batch_ * n_vocab_ * 4, stream_));
     bprompt_ = pr;
     bpen_counts_ = cnt;
-    // one un-captured launch with the current row map (no row, or rows without penalties: every CTA leaves at once) validates the
-    // configuration outside stream capture
-    CU(batch_penalty_launch(8, stream_));
     return {};
 }
 
@@ -208,26 +205,6 @@ Status Engine::keep_prompt(int slot, const int32_t* prompt, int n_prompt) {
     ST(ensure_batch_penalty());
     CU(cudaMemcpyAsync(bprompt_ + (size_t)slot * n_ctx_, prompt, (size_t)n_prompt * 4, cudaMemcpyHostToDevice, stream_));
     return {};
-}
-
-// the penalty kernel over the rows of a batched step (row r: logits row r, the state / history of slot row_slot[r])
-cudaError_t Engine::batch_penalty_launch(int bucket, cudaStream_t s) {
-    PenaltyParams pp{blogits_, n_vocab_, bst_, bctl_, bprompt_, n_ctx_, bout_ids_, max_out_, bpen_counts_};
-    return penalty_launch(pp, bucket, false, s);
-}
-
-// the JSON grammar mask over the rows of a batched step (row r: logits row r, the state of slot row_slot[r]; rows without JSON
-// leave at once)
-cudaError_t Engine::batch_json_launch(int bucket, cudaStream_t s) {
-    JsonMaskParams jp{blogits_, n_vocab_, bst_, bctl_, json_off_, json_bytes_, json_cls_};
-    return json_mask_launch(jp, bucket, false, s);
-}
-
-// the schema mask over the rows of a batched step: rows with a schema follow their SchemaSlot, rows with format json the
-// built-in any-object schema (the JSON mask's result); other rows leave at once
-cudaError_t Engine::batch_schema_launch(int bucket, cudaStream_t s) {
-    SchemaMaskParams sp{blogits_, n_vocab_, bst_, bctl_, sch_ + 1, json_tab_, json_off_, json_bytes_, json_cls_};
-    return schema_mask_launch(sp, bucket, false, s);
 }
 
 // Prefill a prompt into a free slot's own pages and draw its first token.  The single-sequence code runs unchanged on the
@@ -253,8 +230,8 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
     if (!prompt || n_prompt <= 0 || !slot_out) return failb(GL_ERR_INVALID, "seq_open: empty prompt");
     for (int i = 0; i < n_prompt; ++i)
         if (prompt[i] < 0 || prompt[i] >= n_vocab_) return failb(GL_ERR_INVALID, "prompt token id out of range");
-    if (!(so.temperature >= 0.f) || !std::isfinite(so.temperature)) return failb(GL_ERR_INVALID, "temperature must be a finite number >= 0");
-    ST(json_admit(so, false));
+    DrawPlan plan;
+    ST(plan_draw(so, false, &plan));
     ST(ensure_batch_state());
     const int n_pred = so.num_predict > 0 ? so.num_predict : 128;
     if (n_prompt + n_pred > n_ctx_) return failb(GL_ERR_CONTEXT, "prompt + num_predict exceeds the engine context");
@@ -269,9 +246,7 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
     for (int i = 0; i < need; ++i) { S.pages.push_back(free_pages_.back()); free_pages_.pop_back(); }
     int* table = btables_ + (size_t)slot * n_pages_;
     CU(cudaMemcpyAsync(table, S.pages.data(), S.pages.size() * 4, cudaMemcpyHostToDevice, stream_));
-    int penalised = 0;
-    make_state(0, 0, n_prompt, 0, &so, nullptr, &penalised);
-    if (penalised) {                                 // the head of the history the batched steps penalise with
+    if (plan.penalised) {                                 // the head of the history the batched steps penalise with
         Status ks = keep_prompt(slot, prompt, n_prompt);
         if (!ks.ok()) {
             for (int p : S.pages) free_pages_.push_back(p);
@@ -291,11 +266,11 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
         if (ce == cudaSuccess) ce = cudaEventRecord(ev_[2], stream_);
         if (ce != cudaSuccess) { rs = failb(GL_ERR_CUDA, cudaGetErrorString(ce)); break; }
         if (can_batch_prefill(0, n_prompt)) {      // any length: passes of PF_CHUNK rows, the later ones over the slot's pages
-            rs = set_state(n_prompt - 1, prompt[n_prompt - 1], n_prompt, 0, &so);
+            rs = set_state(n_prompt - 1, prompt[n_prompt - 1], n_prompt, 0, &so, plan);
             if (rs.ok()) rs = prefill_batched(0, n_prompt, &dummy);
             if (rs.ok()) rs = enqueue_head(stream_, false, &dummy);
         } else {      // short prompts: plain launches of the decode step (the captured graphs hold the engine's own pointers)
-            rs = set_state(0, prompt[0], n_prompt, 0, &so);
+            rs = set_state(0, prompt[0], n_prompt, 0, &so, plan);
             for (int i = 0; rs.ok() && i < n_prompt; ++i) rs = enqueue_step(stream_, i == n_prompt - 1, false, &dummy);
         }
         if (!rs.ok()) break;
@@ -314,7 +289,6 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
         S.first_lp = lp;
         S.done = hs.done != 0;
     } while (false);
-    const int sampler = sampler_;
     page_table_ = sv.pt; st_ = sv.st; out_ids_ = sv.oi; out_lp_ = sv.ol; host_pos_ = sv.hp;
     if (!rs.ok()) {
         for (int p : S.pages) free_pages_.push_back(p);
@@ -322,9 +296,7 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
         return rs;
     }
     S.open = true;
-    S.n_prompt = n_prompt; S.n_pred = n_pred; S.produced = 0; S.sampler = sampler; S.penalised = penalised; S.first_pending = true;
-    S.json = so.format == GL_FORMAT_JSON ? 1 : so.format >= GL_FORMAT_SCHEMA_BASE ? 2 : 0;
-    S.schema = S.json == 2 ? so.format : 0;
+    S.n_prompt = n_prompt; S.n_pred = n_pred; S.produced = 0; S.plan = plan; S.first_pending = true;
     S.t_open_ns = t_open; S.launches = prefill_launches; S.stopped = S.done;
     bc_[3] += (uint64_t)S.prefill_ns; bc_[4] += (uint64_t)n_prompt; bc_[5] += 1; bc_[6] += (uint64_t)prefill_launches;
     *slot_out = slot;
@@ -341,16 +313,16 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
     if (!ids || !offs || !opts || !slots_out || !n_opened || n_seq <= 0) return failb(GL_ERR_INVALID, "seq_open_many: bad argument");
     *n_opened = 0;
     ST(ensure_batch_state());
+    std::vector<DrawPlan> plans(n_seq);
     for (int i = 0; i < n_seq; ++i) {
         slots_out[i] = -1;
         const int n = offs[i + 1] - offs[i];
         if (n <= 0) return failb(GL_ERR_INVALID, "seq_open_many: empty prompt");
         for (int k = 0; k < n; ++k)
             if (ids[offs[i] + k] < 0 || ids[offs[i] + k] >= n_vocab_) return failb(GL_ERR_INVALID, "prompt token id out of range");
-        if (!(opts[i].temperature >= 0.f) || !std::isfinite(opts[i].temperature)) return failb(GL_ERR_INVALID, "temperature must be a finite number >= 0");
+        ST(plan_draw(opts[i], false, &plans[i]));
         const int n_pred = opts[i].num_predict > 0 ? opts[i].num_predict : 128;
         if (n + n_pred > n_ctx_) return failb(GL_ERR_CONTEXT, "prompt + num_predict exceeds the engine context");
-        ST(json_admit(opts[i], false));
     }
     if (!pk_ids_) {
         auto dalloc = [&](void** p, size_t bytes) -> cudaError_t {
@@ -434,22 +406,18 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             std::vector<StepState> hst(P);
             BatchCtl hc{};
             hc.n_rows = P;
-            bool any_pen = false, any_json = false, any_schema = false;
+            bool any_pen = false, any_mask = false;
             for (int i = 0; i < P && ce == cudaSuccess; ++i) {
                 const int w = which[i], n = lens[i];
-                int sampler = 0, pen = 0;
-                hst[i] = make_state(n - 1, ids[offs[w] + n - 1], n, 0, &opts[w], &sampler, &pen);
-                slots_[pslots[i]].sampler = sampler;
-                slots_[pslots[i]].penalised = pen;
-                slots_[pslots[i]].json = hst[i].json;
-                slots_[pslots[i]].schema = hst[i].json == 2 ? opts[w].format : 0;
-                any_json = any_json || hst[i].json != 0;
-                any_schema = any_schema || hst[i].json == 2;
-                if (hst[i].json == 2) {
-                    Status bs = schema_bind(sch_ + 1 + pslots[i], opts[w].format);
+                const DrawPlan& plan = plans[w];
+                hst[i] = make_state(n - 1, ids[offs[w] + n - 1], n, 0, &opts[w]);
+                slots_[pslots[i]].plan = plan;
+                if (plan.masked) {
+                    Status bs = schema_bind(sch_ + 1 + pslots[i], plan.format);
                     if (!bs.ok()) { rs = bs; break; }
+                    any_mask = true;
                 }
-                if (pen) {                                   // the head of the history the penalty kernel reads
+                if (plan.penalised) {                        // the head of the history the penalty kernel reads
                     Status ks = keep_prompt(pslots[i], ids + offs[w], n);
                     if (!ks.ok()) { rs = ks; break; }
                     any_pen = true;
@@ -461,21 +429,14 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             if (ce == cudaSuccess) ce = cudaMemcpyAsync(bctl_, &hc, sizeof(hc), cudaMemcpyHostToDevice, stream_);
             last_rows_.clear();
             const int bucket = bucket_of(P);
-            if (ce == cudaSuccess && any_pen) {              // penalties before every first-token draw of the pack
-                ce = batch_penalty_launch(bucket, stream_);
-                ++launches;
-            }
-            if (ce == cudaSuccess && any_json) {             // then the JSON grammar mask of the rows that have it (the schema mask
-                ce = any_schema ? batch_schema_launch(bucket, stream_) : batch_json_launch(bucket, stream_);      // when some row has a schema)
-                ++launches;
-            }
+            if (ce == cudaSuccess) ce = enqueue_pre_draw(stream_, bucket, any_pen, any_mask, nullptr, &launches);      // before every first-token draw of the pack
             if (ce == cudaSuccess) ce = batch_sample_greedy_launch(blogits_, n_vocab_, bucket, bctl_, bst_, bout_ids_, bout_lp_, max_out_, bsample_scratch_, stream_);
             for (int i = 0; i < P && ce == cudaSuccess; ++i) {
                 const int slot = pslots[i];
-                if (slots_[slot].sampler != 0) {
+                if (slots_[slot].plan.sampler != 0) {
                     SampleParams sp{blogits_ + (size_t)i * n_vocab_, n_vocab_, bst_ + slot, bout_ids_ + (size_t)slot * max_out_,
                                     bout_lp_ + (size_t)slot * max_out_, nullptr, max_out_, sample_scratch_, topk_scratch_};
-                    ce = sample_topk_launch(sp, slots_[slot].sampler == 1, false, stream_);
+                    ce = sample_topk_launch(sp, slots_[slot].plan.sampler == 1, false, stream_);
                 }
                 if (ce == cudaSuccess)
                     ce = cudaMemcpyAsync(bfirst_logits_ + (size_t)slot * n_vocab_, blogits_ + (size_t)i * n_vocab_, (size_t)n_vocab_ * 4,
@@ -560,7 +521,7 @@ Status Engine::seq_logits(int slot, float* out, int n_vocab) {
 }
 
 // every launch of one batched step, for `bucket` rows; all pointers are fixed, the composition is read from bctl_ / bst_
-Status Engine::enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bool json, int* n_launch, bool schema) {
+Status Engine::enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bool masked, int* n_launch) {
     const int qd = n_head_ * hd_, kvd = n_kv_ * hd_, ldq = qd + 2 * kvd;
     const float scale = 1.0f / std::sqrt((float)hd_);
     int nl = 0;
@@ -641,55 +602,54 @@ Status Engine::enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bo
         const QGemmNorm nm = consume(bssq_[1]);
         CU(linear(bxn16_, head16_, blogits_, n_vocab_, n_embd_, n_vocab_, GEMM_EPI_F32, use_q ? &qhead_ : nullptr, fold ? &nm : nullptr));
     }
-    // repetition penalties of the rows that have them (penalty.cu), before every sampler of the step: only in the variant used
-    // for steps in which some row has penalties
-    if (penalised) { CU(batch_penalty_launch(bucket, s)); ++nl; }
-    // then the JSON grammar mask of the rows that have format json (json_mask.cu): only in the variants used for steps in which
-    // some row has it
-    if (json) { CU(batch_json_launch(bucket, s)); ++nl; }
-    // or the schema mask, for the rows with a schema and those with format json alike (schema_mask.cu): only in the variants
-    // used for steps in which some row has a schema
-    if (schema) { CU(batch_schema_launch(bucket, s)); ++nl; }
+    // repetition penalties, then the grammar mask, of the rows that have them: each only in the variants used for steps in which
+    // some row needs it
+    CU(enqueue_pre_draw(s, bucket, penalised, masked, nullptr, &nl));
     CU(batch_sample_greedy_launch(blogits_, n_vocab_, bucket, bctl_, bst_, bout_ids_, bout_lp_, max_out_, bsample_scratch_, s)); ++nl;
     if (n_launch) *n_launch = nl;
     return {};
 }
 
-// penalised / json: the variants with the penalty kernel / the JSON mask kernel (up to four captured steps per bucket);
+// One un-captured launch of the penalty / mask kernels a new variant adds, on a composition of no rows (every CTA leaves at once;
+// a launch on the real rows would advance their automata), validates their configuration outside stream capture, where an
+// error has a name; the step's composition is restored.
+Status Engine::check_pre_draw(int variant) {
+    const int todo = variant & ~batch_checked_;
+    if (!todo) return {};
+    BatchCtl none{};
+    CU(cudaMemcpyAsync(bctl_, &none, sizeof(int), cudaMemcpyHostToDevice, stream_));
+    cudaError_t e0 = enqueue_pre_draw(stream_, 8, todo & 1, todo & 2);
+    if (e0 == cudaSuccess) e0 = cudaStreamSynchronize(stream_);
+    BatchCtl h{};
+    h.n_rows = (int)last_rows_.size();
+    for (int r = 0; r < h.n_rows; ++r) h.row_slot[r] = last_rows_[r];
+    CU(cudaMemcpyAsync(bctl_, &h, sizeof(h), cudaMemcpyHostToDevice, stream_));
+    CU(cudaStreamSynchronize(stream_));                       // h is on the stack
+    CU(e0);
+    batch_checked_ |= todo;
+    return {};
+}
+
+// penalised / masked: the variants with the penalty kernel / the mask kernel (up to four captured steps per bucket);
 // batch_launches_ counts the plain one
-Status Engine::run_batch_graph(int bucket, bool penalised, bool json, bool schema) {
-    const int bi = bucket_index(bucket);
+Status Engine::run_batch_graph(int bucket, bool penalised, bool masked) {
     if (penalised && !bpen_counts_) return failb(GL_ERR_INVALID, "batched step: no penalty state");
-    if (json && !json_off_) return failb(GL_ERR_INVALID, "batched step: no JSON vocabulary table");
-    if (schema && !sch_) return failb(GL_ERR_INVALID, "batched step: no schema state");
-    const int extra = (penalised ? 1 : 0) + (json ? 1 : 0) + (schema ? 1 : 0);
+    if (masked && !sch_) return failb(GL_ERR_INVALID, "batched step: no mask state");
+    const int variant = (penalised ? 1 : 0) | (masked ? 2 : 0);
+    const int extra = (penalised ? 1 : 0) + (masked ? 1 : 0);
     if (!use_graph_) {
         int nl = 0;
-        ST(enqueue_batch_step(stream_, bucket, penalised, json, &nl, schema));
+        ST(enqueue_batch_step(stream_, bucket, penalised, masked, &nl));
         batch_launches_ = nl - extra;
         return {};
     }
-    cudaGraphExec_t& ge = g_batch_[bi][(penalised ? 1 : 0) | (json ? 2 : 0) | (schema ? 4 : 0)];
+    cudaGraphExec_t& ge = g_batch_[bucket_index(bucket)][variant];
     if (!ge) {
-        if ((json && !batch_json_checked_) || (schema && !batch_schema_checked_)) {
-            // one un-captured launch on a composition of no rows (every CTA leaves at once; a launch on the real rows would
-            // advance their automata) validates the configuration outside stream capture; the step's composition is restored
-            BatchCtl none{};
-            CU(cudaMemcpyAsync(bctl_, &none, sizeof(int), cudaMemcpyHostToDevice, stream_));
-            cudaError_t e0 = json ? batch_json_launch(8, stream_) : batch_schema_launch(8, stream_);
-            if (e0 == cudaSuccess) e0 = cudaStreamSynchronize(stream_);
-            BatchCtl h{};
-            h.n_rows = (int)last_rows_.size();
-            for (int r = 0; r < h.n_rows; ++r) h.row_slot[r] = last_rows_[r];
-            CU(cudaMemcpyAsync(bctl_, &h, sizeof(h), cudaMemcpyHostToDevice, stream_));
-            CU(cudaStreamSynchronize(stream_));                       // h is on the stack
-            CU(e0);
-            (json ? batch_json_checked_ : batch_schema_checked_) = true;
-        }
+        ST(check_pre_draw(variant));
         cudaGraph_t g = nullptr;
         int nl = 0;
         CU(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
-        Status st = enqueue_batch_step(stream_, bucket, penalised, json, &nl, schema);
+        Status st = enqueue_batch_step(stream_, bucket, penalised, masked, &nl);
         cudaError_t e = cudaStreamEndCapture(stream_, &g);
         if (!st.ok()) { if (g) cudaGraphDestroy(g); return st; }
         if (e != cudaSuccess) return failb(GL_ERR_CUDA, std::string("batched step: graph capture: ") + cudaGetErrorString(e));
@@ -749,22 +709,20 @@ Status Engine::batch_step(int32_t* out_slots, int32_t* out_ids, float* out_lps, 
         last_rows_ = rows;
     }
     last_bucket_ = bucket;
-    bool penalised = false, json = false, schema = false;     // the step with the penalty / a mask kernel only when some row needs it
+    bool penalised = false, masked = false;         // the step with the penalty / mask kernel only when some row needs it
     for (int r = 0; r < B; ++r) {
-        penalised = penalised || slots_[rows[r]].penalised != 0;
-        json = json || slots_[rows[r]].json != 0;
-        schema = schema || slots_[rows[r]].json == 2;
+        penalised = penalised || slots_[rows[r]].plan.penalised;
+        masked = masked || slots_[rows[r]].plan.masked;
     }
-    if (schema) json = false;                        // the schema mask masks the format json rows too
     CU(cudaEventRecord(ev_[2], stream_));
-    ST(run_batch_graph(bucket, penalised, json, schema));
-    const int step_launches = batch_launches_ + (penalised ? 1 : 0) + (json || schema ? 1 : 0) + 1;
+    ST(run_batch_graph(bucket, penalised, masked));
+    const int step_launches = batch_launches_ + (penalised ? 1 : 0) + (masked ? 1 : 0) + 1;
     for (int r = 0; r < B; ++r) {                    // sampled rows: the seeded top-k / top-p sampler of the single-sequence path
         const int slot = rows[r];
-        if (slots_[slot].sampler == 0) continue;
+        if (slots_[slot].plan.sampler == 0) continue;
         SampleParams sp{blogits_ + (size_t)r * n_vocab_, n_vocab_, bst_ + slot, bout_ids_ + (size_t)slot * max_out_, bout_lp_ + (size_t)slot * max_out_,
                         nullptr, max_out_, sample_scratch_, topk_scratch_};
-        CU(sample_topk_launch(sp, slots_[slot].sampler == 1, false, stream_));
+        CU(sample_topk_launch(sp, slots_[slot].plan.sampler == 1, false, stream_));
     }
     CU(batch_collect_launch(bctl_, bst_, bout_lp_, max_out_, bout_, bucket, stream_));
     CU(cudaEventRecord(ev_[3], stream_));

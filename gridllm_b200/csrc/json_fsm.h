@@ -11,7 +11,7 @@
 //   ws      ::= "" | " " | "\n" [ \t]{0,20}
 //
 // with nesting depth <= JSON_MAX_DEPTH (root included).  The grammar never puts two ws slots side by side, so one counter
-// tracks the current slot.  Everything is __host__ __device__: the mask kernel (json_mask.cu) runs exactly this program per
+// tracks the current slot.  Everything is __host__ __device__: the mask kernel (schema_mask.cu) runs exactly this program per
 // vocabulary entry, the host validates histories with it (gl_constrain_logits), and tests/test_json_cpu.py compiles it with g++
 // and checks it state for state against the Python restatement.
 #pragma once
@@ -239,7 +239,7 @@ JSON_HD bool json_run(JsonState& s, const uint8_t* p, int n) {
     return true;
 }
 
-// per-token class bit (json_mask.cu): every byte is printable ASCII other than '"' and '\' -- such a token is accepted whole in
+// per-token class bit (schema_mask.cu): every byte is printable ASCII other than '"' and '\' -- such a token is accepted whole in
 // the string-body state without the byte loop
 constexpr uint8_t JSON_CLS_PLAIN = 1;
 

@@ -166,41 +166,25 @@ struct PenaltyParams {
 };
 cudaError_t penalty_launch(const PenaltyParams& p, int rows, bool pdl, cudaStream_t s);
 
-// JSON grammar mask in place on the logits, after the penalties and before the sampler (json_mask.cu; language in json_fsm.h,
-// semantics in include/gridllm_native.h).  Grid: vocabulary chunks x rows, one thread per token.  A row's automaton state
-// lives in its StepState (json_st, two entries by output-index parity); rows without JSON and finished rows leave at once.
-struct JsonMaskParams {
-    float* logits;              // row r at logits + r * n_vocab
-    int n_vocab;
-    StepState* st;              // ctl == null: the one sequence's state; else [slots]
-    const BatchCtl* ctl;        // batched step: row -> slot, rows >= n_rows leave at once; null: one row, slot 0
-    const uint32_t* offsets;    // [n_vocab + 1] byte offsets of the token pieces
-    const uint8_t* bytes;       // the pieces, back to back
-    const uint8_t* cls;         // [n_vocab] class bits (JSON_CLS_*)
-};
-cudaError_t json_mask_launch(const JsonMaskParams& p, int rows, bool pdl, cudaStream_t s);
-// one thread: the automaton from the initial state through the pieces of ids[0..n-1) (all but the last), stored as the entry
-// the mask kernel of output n reads; that kernel then advances by ids[n-1] (= st->token) itself.  gl_constrain_logits.
-cudaError_t json_replay_launch(StepState* st, const int* ids, int n, const uint32_t* offsets, const uint8_t* bytes, cudaStream_t s);
-
-// JSON schema mask (schema_mask.cu; language in schema_fsm.h, semantics in include/gridllm_native.h gl_format_schema): the grid
-// of json_mask_launch.  Rows with StepState.json = 2 follow their SchemaSlot; rows with json = 1 (format json) follow the
-// built-in any-object schema from their json_st, giving json_mask_launch's mask; other rows and finished rows leave at once.
+// JSON grammar mask in place on the logits, after the penalties and before the sampler (schema_mask.cu; language in
+// schema_fsm.h over json_fsm.h, semantics in include/gridllm_native.h: format json and gl_format_schema).  Grid: vocabulary
+// chunks x rows, one thread per token.  Rows with StepState.json = 1 follow the schema their SchemaSlot points at (format json:
+// the built-in any-object schema); other rows and finished rows leave at once.
 struct SchemaSlot {
     const uint8_t* tab;         // the row's compiled schema (schema_compile.cpp blob), set by the host when the request starts
     uint32_t pad[2];
-    SchemaState st[2];          // st[i & 1]: the automaton state after the output's first i tokens (as StepState.json_st)
+    SchemaState st[2];          // st[i & 1]: the automaton state after the output's first i tokens (written by the mask kernel
+                                // of output i, read by that of output i + 1)
 };
 struct SchemaMaskParams {
     float* logits;              // row r at logits + r * n_vocab
     int n_vocab;
     StepState* st;              // ctl == null: the one sequence's state; else [slots]
-    const BatchCtl* ctl;        // batched step: row -> slot; null: one row
+    const BatchCtl* ctl;        // batched step: row -> slot, rows >= n_rows leave at once; null: one row
     SchemaSlot* ss;             // ctl == null: the one sequence's entry; else [slots]
-    const uint8_t* json_tab;    // the built-in any-object schema
-    const uint32_t* offsets;    // the vocabulary table of JsonMaskParams
-    const uint8_t* bytes;
-    const uint8_t* cls;
+    const uint32_t* offsets;    // [n_vocab + 1] byte offsets of the token pieces
+    const uint8_t* bytes;       // the pieces, back to back
+    const uint8_t* cls;         // [n_vocab] class bits (JSON_CLS_*)
 };
 cudaError_t schema_mask_launch(const SchemaMaskParams& p, int rows, bool pdl, cudaStream_t s);
 // one thread: e's automaton from the initial state through the pieces of ids[0..n-1), stored as entry (n - 1) & 1 (the mask

@@ -378,15 +378,6 @@ JSON_HD bool schema_step(const SchemaView& v, JsonState& js, SchemaCursor& cur, 
     }
 }
 
-// The state of a row of the built-in any-object schema (format json) from its JsonState alone: the cursor follows from the mode.
-JSON_HD void schema_cursor_of_json(const JsonState& js, const SchemaView& v, SchemaCursor& cur) {
-    cur = SchemaCursor{};
-    cur.node = (uint16_t)v.root;
-    if (js.mode == JM_START) cur.phase = SP_VALUE;
-    else if (js.depth == 0 && js.mode == JM_AFTER) cur.phase = SP_CONT;
-    else { cur.phase = SP_ANY; cur.base = 0; }
-}
-
 JSON_HD bool schema_done(const JsonState& js) { return json_done(js); }
 
 template <class F>

@@ -1,18 +1,21 @@
-// JSON schema mask on the device (Ollama's `format` as a JSON schema).  Language: schema_fsm.h over json_fsm.h; semantics:
-// gl_format_schema in include/gridllm_native.h; restated in tests/schema_oracle.py.
+// JSON grammar mask on the device: Ollama's `format`, either "json" or a JSON schema.  Language: schema_fsm.h over json_fsm.h;
+// semantics: gl_sample_opts.format and gl_format_schema in include/gridllm_native.h; restated in tests/json_oracle.py and
+// tests/schema_oracle.py.  Format json is the built-in any-object schema, so one kernel masks both kinds of row.
 //
-// The grid of json_mask_kernel: vocabulary chunks of SM_THREADS x rows, one thread per token.  A row with a schema
-// (StepState.json = 2) keeps its automaton state in its SchemaSlot (two entries by output parity, like StepState.json_st) and
-// finds its tables through the slot's pointer, so one captured graph serves any mix of schemas.  A row with format json
-// (StepState.json = 1) is the built-in any-object schema: its state stays the JsonState in StepState.json_st (the one
-// json_mask_kernel keeps), from which the cursor follows, so the two kernels can take turns on the same row and give identical
-// masks.
+// Grid (vocabulary chunks of SM_THREADS) x rows, one thread per token.  A masked row (StepState.json = 1) keeps its automaton
+// state in its SchemaSlot (two entries by output parity) and finds its tables through the slot's pointer, so one captured graph
+// serves any mix of schemas.  The CTA loads the row's state into shared memory, thread 0 advances it by the piece of the token
+// drawn last (StepState.token; output 0 starts from the initial state), and CTA 0 stores the result as the entry of this
+// output, which only the next launch reads: no CTA reads what another CTA of the same launch writes, and a captured graph
+// replays with no host.  Every thread then walks its token's piece from the shared state with a private JsonState and cursor
+// and a private overlay of the frames it touches (it copies a frame from shared memory the first time it needs it; it only ever
+// needs the top one or pushes a new one), which is exact for any piece length, and writes -inf on rejection.  Stop tokens (the
+// row's stop_ids: eos / eot / the request's) are allowed exactly when the document has closed; other empty pieces (control
+// tokens) never.  Plain string text (JSON_CLS_PLAIN) passes an unbounded string without the byte loop.
 //
-// The CTA loads the row's state into shared memory, thread 0 advances it by the piece of the token drawn last, and CTA 0 stores
-// the result as the entry of this output.  Every thread then walks its token's piece from the shared state with a private
-// JsonState and cursor and a private overlay of the frames it touches (it copies a frame from shared memory the first time it
-// needs it; it only ever needs the top one or pushes a new one), which is exact for any piece length.  Plain string text takes
-// the fast path of json_mask_kernel where the string is unbounded.
+// Bound: latency -- one launch, one L2 round trip for the offsets and a few for the piece bytes (1-2 MB of table for a 128 k
+// vocabulary, resident in L2 after the first step), n_vocab logit writes at most.  The host only puts the kernel into steps
+// where some row is masked: one extra launch per draw.
 #include "common.cuh"
 #include "kernels.h"
 #include "batch.h"
@@ -56,13 +59,11 @@ __global__ void __launch_bounds__(SM_THREADS) schema_mask_kernel(const __grid_co
         slot = __ldcg(&p.ctl->row_slot[row]);
     }
     StepState* st = p.st + slot;
-    const int kind = __ldcg(&st->json);
-    if (!kind || __ldcg(&st->done)) return;
+    if (!__ldcg(&st->json) || __ldcg(&st->done)) return;
     SchemaSlot* e = p.ctl ? p.ss + slot : p.ss;
     const int out_idx = __ldcg(&st->out_idx);
-    const uint8_t* tab = kind == 1 ? p.json_tab : (const uint8_t*)__ldcg((const unsigned long long*)&e->tab);
-    const SchemaView v = schema_view(tab);
-    if (kind == 2 && out_idx > 0) {
+    const SchemaView v = schema_view((const uint8_t*)__ldcg((const unsigned long long*)&e->tab));
+    if (out_idx > 0) {
         const unsigned* src = reinterpret_cast<const unsigned*>(&e->st[(out_idx - 1) & 1]);
         unsigned* dst = reinterpret_cast<unsigned*>(&s_state);
         for (int k = threadIdx.x; k < SM_STATE_WORDS; k += SM_THREADS) dst[k] = __ldcg(src + k);
@@ -70,23 +71,7 @@ __global__ void __launch_bounds__(SM_THREADS) schema_mask_kernel(const __grid_co
     __syncthreads();
     if (threadIdx.x == 0) {
         const int prev = out_idx > 0 ? __ldcg(&st->token) : -1;
-        if (kind == 1) {                                             // format json: the JsonState of json_mask_kernel
-            JsonState js{};
-            if (out_idx > 0) {
-                unsigned* d = reinterpret_cast<unsigned*>(&js);
-                for (int k = 0; k < 4; ++k) d[k] = __ldcg(&st->json_st[(out_idx - 1) & 1][k]);
-                if ((unsigned)prev < (unsigned)p.n_vocab) {
-                    const uint32_t a = __ldg(p.offsets + prev), b = __ldg(p.offsets + prev + 1);
-                    json_run(js, p.bytes + a, (int)(b - a));
-                }
-            }
-            if (blockIdx.x == 0) {
-                const unsigned* d = reinterpret_cast<const unsigned*>(&js);
-                for (int k = 0; k < 4; ++k) st->json_st[out_idx & 1][k] = d[k];
-            }
-            s_state.js = js;
-            schema_cursor_of_json(js, v, s_state.cur);
-        } else if (out_idx == 0) {
+        if (out_idx == 0) {
             schema_init(s_state.js, s_state.cur, v);
         } else if ((unsigned)prev < (unsigned)p.n_vocab) {
             SchemaArrayFrames fr{s_state.fr};
@@ -97,7 +82,7 @@ __global__ void __launch_bounds__(SM_THREADS) schema_mask_kernel(const __grid_co
         for (int k = 0; k < ns; ++k) s_stop[k] = __ldcg(&st->stop_ids[k]);
     }
     __syncthreads();
-    if (kind == 2 && blockIdx.x == 0) {
+    if (blockIdx.x == 0) {
         const unsigned* src = reinterpret_cast<const unsigned*>(&s_state);
         unsigned* dst = reinterpret_cast<unsigned*>(&e->st[out_idx & 1]);
         for (int k = threadIdx.x; k < SM_STATE_WORDS; k += SM_THREADS) dst[k] = src[k];
@@ -140,7 +125,7 @@ __global__ void schema_replay_kernel(SchemaSlot* e, const int* ids, int n, const
 }  // namespace
 
 cudaError_t schema_mask_launch(const SchemaMaskParams& p, int rows, bool pdl, cudaStream_t s) {
-    if (!p.logits || !p.st || !p.ss || !p.json_tab || !p.offsets || !p.bytes || !p.cls || rows < 1 || p.n_vocab < 1) return cudaErrorInvalidValue;
+    if (!p.logits || !p.st || !p.ss || !p.offsets || !p.bytes || !p.cls || rows < 1 || p.n_vocab < 1) return cudaErrorInvalidValue;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;

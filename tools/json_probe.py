@@ -1,4 +1,4 @@
-"""Cost of the JSON grammar mask (format: "json", json_mask.cu) on the Llama-3-8B-shaped synthetic model with its synthetic
+"""Cost of the JSON grammar mask (format: "json", schema_mask.cu over the built-in any-object schema) on the Llama-3-8B-shaped synthetic model with its synthetic
 vocabulary (256 byte tokens, a few dozen merges, <filler_N> pieces -- not Llama-3's, so the bytes per token differ from a real
 model's):
   - decode device time per token, 512 in / 128 out, greedy vs greedy + JSON and top_k 40 vs top_k 40 + JSON, the cases
@@ -73,7 +73,7 @@ def _mask_kernel_time(e, prompt, seed):
     durs = {}
     for ev in prof.events():
         name = ev.name
-        for k in ("json_mask_kernel", "sample_topk_fast_kernel", "gemv_kernel"):
+        for k in ("schema_mask_kernel", "sample_topk_fast_kernel", "gemv_kernel"):
             if k in name:
                 durs.setdefault(k, []).append(getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0.0))
     for name, d in durs.items():

@@ -3,7 +3,8 @@ vocabulary (not Llama-3's: the bytes per token differ from a real model's):
   - decode device time per token, 512 in / 128 out: no format / format "json" / a pydantic-style nested schema, greedy and
     top_k 40, the cases interleaved round by round, best of the rounds (eval_count is printed: a request may end early);
   - one batched step at B = 32 (top_k 40 rows), every row on the schema vs none, when enough prompts keep the document open;
-  - the schema kernel's own device time per launch, from a torch.profiler (CUPTI) trace (beside json_mask_kernel's);
+  - the mask kernel's own device time per launch on schema rows, from a torch.profiler (CUPTI) trace (tools/json_probe.py
+    times it on format json rows);
   - host compile time of gl_format_schema on the schemas of tests/test_schema_cpu.py.
 Requests are timed on prompts / seeds for which the document stays open for all 128 tokens (found by trying them).  The first
 line names the card, its power limit and its maximum SM clock."""
@@ -75,12 +76,12 @@ def _kernel_time(e, prompt, seed):
     from torch.profiler import ProfilerActivity, profile
     torch.cuda.init()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for fmt in (SCHEMA, "json"):
+        for fmt in (SCHEMA,):
             for _ in range(3):
                 e.generate(prompt, num_predict=64, format=fmt, seed=seed, **SAMP)
     durs = {}
     for ev in prof.events():
-        for k in ("schema_mask_kernel", "json_mask_kernel", "sample_topk_fast_kernel"):
+        for k in ("schema_mask_kernel", "sample_topk_fast_kernel"):
             if k in ev.name:
                 durs.setdefault(k, []).append(getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0.0))
     for name, d in durs.items():
