@@ -3,23 +3,27 @@
 // Stands in for the attention inside Ollama's decode step, reached in the reference only through
 // OllamaService.generate*Response (/root/reference/client/src/services/OllamaService.ts:142-145, 235-237).
 // Bound: HBM (KV pages) in principle, latency in practice at the 512+128-token workloads of BASELINE.json (2.6 MB
-// of KV per layer), so everything is arranged to shorten the dependent chain: one launch; split s owns pages s, s+S,
-// ... (independent of the context length), so the pages that are already final are staged with 1-D TMA bulk copies
-// BEFORE griddepcontrol.wait, while the QKV GEMV that appends the newest row is still running (a 16-token page of one
-// KV head is one contiguous 4 KB block); after the wait only the page holding the newest rows is fetched; per page a
-// transposing 16-shuffle score reduction; partials merged by the last CTA of each KV head (atomic ticket) with
-// batched loads -- no second kernel.  The grid is fixed (it lives in a CUDA graph); surplus splits leave at once,
-// and a context of one page is written straight to the output without partials, ticket or merge.
+// of KV per layer), so everything is arranged to shorten the dependent chain after griddepcontrol.wait:
+// * one launch; the S splits of a KV head are ONE thread-block cluster; split s owns pages s, s+S, ... (independent of the
+//   context length), so every row that is already final -- whole pages and the leading rows of the newest page -- is
+//   staged with 1-D TMA bulk copies BEFORE the wait, while the QKV GEMV that appends the newest row is still running;
+// * after the wait ONE round trip: q, the position and the newest K / V row (the one the QKV epilogue just appended,
+//   fetched at the position read before the wait) are requested together;
+// * two warps per query head, each walking half of the split's pages, merged in shared memory; the splits merge through
+//   distributed shared memory (every split sends each rank the slice of its partial that rank merges, one cluster
+//   barrier): no global partials, no atomic ticket, no last-CTA merge.  Splits are merged in rank order: deterministic.
+// The grid is fixed (it lives in a CUDA graph); surplus splits only join the barrier, and a context of one page is
+// written straight to the output by split 0 without any merge.
 #include "attn_core.cuh"
 
 namespace gl {
 
 namespace {
 
-constexpr int TILE_PAGES = 4;
+constexpr int STAGE_PAGES = 8;      // pages per split staged at once (before the wait: every final page up to 16 * S * 8 tokens)
 constexpr int MAX_GRP = 8;
-
-constexpr int MAX_CL = 16;          // splits of one KV head in one thread-block cluster (cluster mode)
+constexpr int WPH = 2;              // warps per query head
+constexpr int MAX_CL = 16;          // splits of one KV head = CTAs of one cluster
 
 __device__ __forceinline__ uint32_t attn_mapa(uint32_t local_smem_addr, uint32_t rank) {      // the same location in CTA `rank` of the cluster
     uint32_t ra;
@@ -27,28 +31,51 @@ __device__ __forceinline__ uint32_t attn_mapa(uint32_t local_smem_addr, uint32_t
     return ra;
 }
 
-// CL = false: partials through global memory, merged by the last CTA of each KV head (atomic ticket).
-// CL = true : the n_splits CTAs of a KV head are ONE thread-block cluster.  Every split sends each rank the slice of its partial
-//             output that rank owns (st.shared::cluster into the rank's receive buffer: distributed shared memory) with its
-//             (max, sum); one cluster barrier; every rank merges its slice of the head group's output -- no global round trip,
-//             no ticket, and the merge is spread over the cluster (the ticket path: partial store 0.9 us + ticket 0.8 us + the
-//             last CTA's 32 partial loads 2.0 us per layer).
-template <int DPL, bool CL>   // dims per lane = head_dim / 32
-__global__ void __launch_bounds__(32 * MAX_GRP) attn_decode_kernel(const __grid_constant__ AttnParams p) {
+template <int DPL>
+__device__ __forceinline__ uint2 ld_row(const __half* p) {      // this lane's DPL dims of one K / V row, through L2
+    if (DPL == 4) return __ldcg(reinterpret_cast<const uint2*>(p));
+    return make_uint2(__ldcg(reinterpret_cast<const unsigned*>(p)), 0u);
+}
+template <int DPL>
+__device__ __forceinline__ uint2 lds_row(const __half* p) {
+    if (DPL == 4) return *reinterpret_cast<const uint2*>(p);
+    return make_uint2(*reinterpret_cast<const unsigned*>(p), 0u);
+}
+
+// One page against one query head, rows from shared memory except row `jn` (-1: none), which this lane holds in kn / vn.
+template <int DPL>
+__device__ __forceinline__ void page_math(const __half* kb, const __half* vb, int npos, int jn, uint2 kn, uint2 vn, const float* q, float* o,
+                                          float& m_run, float& l_run) {
+    constexpr int HD = DPL * 32;
+    uint2 kk[KV_PAGE_TOKENS];
+#pragma unroll
+    for (int j = 0; j < KV_PAGE_TOKENS; ++j) kk[j] = j == jn ? kn : lds_row<DPL>(kb + j * HD);
+    const float w = attn_page_scores<DPL>(kk, npos, q, o, m_run, l_run);
+#pragma unroll
+    for (int j = 0; j < KV_PAGE_TOKENS; ++j) {
+        if (j >= npos) break;                                      // warp-uniform; rows beyond npos may hold anything
+        attn_pv_row<DPL>(w, j, j == jn ? vn : lds_row<DPL>(vb + j * HD), o);
+    }
+}
+
+// grid (n_kv_heads, S), cluster (1, S, 1), 32 * WPH * grp threads: warp = half * grp + head of the group
+template <int DPL>
+__global__ void __launch_bounds__(32 * WPH * MAX_GRP) attn_decode_kernel(const __grid_constant__ AttnParams p) {
     constexpr int HD = DPL * 32;
     constexpr int PAGE_ELEMS = KV_PAGE_TOKENS * HD;
-    constexpr uint32_t PAGE_BYTES = PAGE_ELEMS * sizeof(__half);
-    __shared__ __align__(128) __half ks[TILE_PAGES * PAGE_ELEMS];
-    __shared__ __align__(128) __half vs[TILE_PAGES * PAGE_ELEMS];
+    constexpr uint32_t ROW_BYTES = HD * sizeof(__half);
+    extern __shared__ __align__(128) __half stage_buf[];           // [STAGE_PAGES][K page, V page]
     __shared__ __align__(8) uint64_t bar;
-    __shared__ int is_last;
-    __shared__ __align__(16) float rx_o[CL ? MAX_CL : 1][CL ? 128 : 4];      // [split][this rank's slice of the group's output]
-    __shared__ __align__(8) float rx_ml[CL ? MAX_CL : 1][2];                 // [split](max, sum) of the head the slice belongs to
+    __shared__ __align__(16) float pair_o[MAX_GRP][HD];             // the second warp of each head: its partial
+    __shared__ float pair_ml[MAX_GRP][2];
+    __shared__ __align__(16) float rx_o[MAX_CL][128];               // [split][this rank's slice of the group's output]
+    __shared__ __align__(8) float rx_ml[MAX_CL][MAX_GRP][2];        // [split][head of the group](max, sum)
 
-    const int kvh = blockIdx.x, split = blockIdx.y;
+    const int kvh = blockIdx.x, split = blockIdx.y;                 // cluster (1, S, 1): split = rank in the cluster
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int grp = p.n_head / p.n_kv_heads;
-    const int head = kvh * grp + warp;
+    const int hw = warp % grp, half = warp / grp;
+    const int head = kvh * grp + hw;
     const int S = p.n_splits;
 
     if (threadIdx.x == 0) {
@@ -61,31 +88,34 @@ __global__ void __launch_bounds__(32 * MAX_GRP) attn_decode_kernel(const __grid_
     __syncthreads();
     pdl_launch_dependents();
 
-    // Split s owns pages s, s + S, s + 2S, ... -- a mapping that does not depend on the context length, so the pages
-    // that are already FINAL can be requested before the upstream kernel (this layer's QKV GEMV, which appends the
-    // newest row) has finished: the position counter only grows inside a sequence, so any value read here is a lower
-    // bound, and a page whose 16 rows all lie below it was completed by earlier steps.
+    // The position counter only grows inside a sequence, so a value read before the wait is a lower bound pos_lb: every
+    // row below it was appended by an earlier step, whose kernels have completed, and is final.  Only rows < pos_lb are
+    // requested here.  Row pos_lb is written by the upstream QKV epilogue (or, if pos_lb is stale, by an earlier step that
+    // may still be running); it is read only after the wait, and used only when the position read after the wait is pos_lb.
     const int pos_lb = __ldcg(&p.st->pos);
-    const int final_pages = pos_lb / KV_PAGE_TOKENS;
-    int npre = 0;
-    if (split < final_pages) npre = min(TILE_PAGES, (final_pages - split + S - 1) / S);
-    // lane i's page-table entry of this split's i-th page: static, requested before the wait (clamped to the table)
-    int my_entry = 0;
-    if (warp == 0 && lane < TILE_PAGES) my_entry = __ldcg(p.page_table + min(split + lane * S, p.n_table - 1));
-    auto stage = [&](int slot, int page) {        // one lane: two bulk copies of a physical page
+    const int lb_pages = (pos_lb + KV_PAGE_TOKENS - 1) / KV_PAGE_TOKENS;      // pages holding at least one row < pos_lb
+    const int npre = split < lb_pages ? min(STAGE_PAGES, (lb_pages - split + S - 1) / S) : 0;
+    const int new_pg = pos_lb / KV_PAGE_TOKENS;                     // page of row pos_lb
+    const bool own_new = new_pg % S == split;
+    const int new_entry = own_new ? __ldcg(p.page_table + min(new_pg, p.n_table - 1)) : 0;
+    int my_entry = 0;                                               // lane i of warp 0: this split's i-th page
+    if (warp == 0 && lane < STAGE_PAGES) my_entry = __ldcg(p.page_table + min(split + lane * S, p.n_table - 1));
+    auto stage = [&](int slot, int page, int rows) {                // one lane: two bulk copies of the first `rows` rows of a page
         const size_t off = ((size_t)page * p.n_kv_heads + kvh) * PAGE_ELEMS;
-        tma_load_1d(ks + slot * PAGE_ELEMS, p.k_cache + off, PAGE_BYTES, &bar);
-        tma_load_1d(vs + slot * PAGE_ELEMS, p.v_cache + off, PAGE_BYTES, &bar);
+        tma_load_1d(stage_buf + slot * 2 * PAGE_ELEMS, p.k_cache + off, rows * ROW_BYTES, &bar);
+        tma_load_1d(stage_buf + slot * 2 * PAGE_ELEMS + PAGE_ELEMS, p.v_cache + off, rows * ROW_BYTES, &bar);
     };
     if (warp == 0 && npre > 0) {
-        if (lane == 0) mbar_expect_tx(&bar, 2u * npre * PAGE_BYTES);
+        const int rows = lane < npre ? min(KV_PAGE_TOKENS, pos_lb - (split + lane * S) * KV_PAGE_TOKENS) : 0;
+        const unsigned total = __reduce_add_sync(0xffffffffu, (unsigned)rows);
+        if (lane == 0) mbar_expect_tx(&bar, 2u * total * ROW_BYTES);
         __syncwarp();
-        if (lane < npre) stage(lane, my_entry);
+        if (lane < npre) stage(lane, my_entry, rows);
     }
     pdl_wait();
     if (tr) tr[1] = globaltimer_ns();
 
-    // q and the position travel together (a warp issues in order: nothing below may consume the position before q is requested)
+    // one round trip: q, the position and (speculatively, at pos_lb) the newest K / V row travel together
     float q[DPL], o[DPL];
     {
         const float* qp = p.q + (size_t)head * HD + lane * DPL;
@@ -99,140 +129,139 @@ __global__ void __launch_bounds__(32 * MAX_GRP) attn_decode_kernel(const __grid_
 #pragma unroll
         for (int d = 0; d < DPL; ++d) o[d] = 0.f;
     }
-    const int L = __ldcg(&p.st->pos) + 1;
+    uint2 kn = make_uint2(0u, 0u), vn = make_uint2(0u, 0u);
+    if (own_new) {
+        const size_t off = ((size_t)new_entry * p.n_kv_heads + kvh) * PAGE_ELEMS + (size_t)(pos_lb % KV_PAGE_TOKENS) * HD + lane * DPL;
+        kn = ld_row<DPL>(p.k_cache + off);
+        vn = ld_row<DPL>(p.v_cache + off);
+    }
+    const int pos = __ldcg(&p.st->pos);
+    const int L = pos + 1;
 #pragma unroll
     for (int d = 0; d < DPL; ++d) q[d] *= p.scale;
     const int n_pages = (L + KV_PAGE_TOKENS - 1) / KV_PAGE_TOKENS;
     const int active = min(n_pages, S);
-    if (!CL && split >= active) return;             // (then nothing was staged either: final_pages <= n_pages)
-    const int my_pages = split < active ? (n_pages - split + S - 1) / S : 0;      // cluster mode: idle splits stay for the barrier
+    const int my_pages = split < active ? (n_pages - split + S - 1) / S : 0;
+    const bool fresh = pos == pos_lb;                               // else rows >= pos_lb are (re)fetched after the wait
 
     float m_run = -INFINITY, l_run = 0.f;
     uint32_t ph = 0;
-    for (int t0 = 0; t0 < my_pages; t0 += TILE_PAGES) {
-        const int np = min(TILE_PAGES, my_pages - t0);
-        const int have = t0 == 0 ? npre : 0;        // pages of this tile already requested before the wait
+    for (int t0 = 0; t0 < my_pages; t0 += STAGE_PAGES) {
+        const int np = min(STAGE_PAGES, my_pages - t0);
+        const int have = t0 == 0 ? npre : 0;                        // pages of this tile requested before the wait
+        // pages still to fetch: every page of a later tile; in the first tile none when the position is pos_lb (row pos_lb
+        // is in registers), else each page holding a row >= pos_lb, whole (its pre-wait rows are fetched again)
+        const int first = t0 > 0 ? 0 : fresh ? np : min(np, max(0, (pos_lb / KV_PAGE_TOKENS - split + S - 1) / S));
         if (have > 0) { mbar_wait(&bar, ph); ph ^= 1; }
-        if (np > have) {                            // the rest: the page holding the newest rows (and long contexts)
-            // every thread must have seen the previous phase complete before the barrier is armed again: a straggler
-            // that still waits for parity p when phase p+1 completes would wait for ever (parity aliasing)
-            if (have > 0) __syncthreads();
+        if (first < np) {
+            // every thread must have seen the previous phase complete before the barrier is armed again (parity aliasing),
+            // and the staging slots of the previous tile must be consumed
+            if (have > 0 || t0 > 0) __syncthreads();
             if (warp == 0) {
-                if (lane == 0) mbar_expect_tx(&bar, 2u * (np - have) * PAGE_BYTES);
+                const int i = t0 + lane;
+                const int pg = split + i * S;
+                const int rows = lane >= first && lane < np ? min(KV_PAGE_TOKENS, L - pg * KV_PAGE_TOKENS) : 0;
+                const unsigned total = __reduce_add_sync(0xffffffffu, (unsigned)rows);
+                if (lane == 0) mbar_expect_tx(&bar, 2u * total * ROW_BYTES);
                 __syncwarp();
-                if (lane >= have && lane < np) stage(lane, t0 == 0 ? my_entry : __ldcg(p.page_table + split + (t0 + lane) * S));
+                if (rows > 0) stage(lane, t0 == 0 ? my_entry : __ldcg(p.page_table + pg), rows);
             }
             mbar_wait(&bar, ph);
             ph ^= 1;
         }
-        for (int i = 0; i < np; ++i) {
-            uint2 kk[KV_PAGE_TOKENS], vv[KV_PAGE_TOKENS];
-            const __half* kb = ks + i * PAGE_ELEMS + lane * DPL;
-            const __half* vb = vs + i * PAGE_ELEMS + lane * DPL;
-#pragma unroll
-            for (int j = 0; j < KV_PAGE_TOKENS; ++j) {
-                if (DPL == 4) {
-                    kk[j] = *reinterpret_cast<const uint2*>(kb + j * HD);
-                    vv[j] = *reinterpret_cast<const uint2*>(vb + j * HD);
-                } else {
-                    kk[j] = make_uint2(*reinterpret_cast<const unsigned*>(kb + j * HD), 0u);
-                    vv[j] = make_uint2(*reinterpret_cast<const unsigned*>(vb + j * HD), 0u);
-                }
-            }
+        for (int i = half; i < np; i += WPH) {
             const int pg = split + (t0 + i) * S;
-            attn_page_math<DPL>(kk, vv, min(KV_PAGE_TOKENS, L - pg * KV_PAGE_TOKENS), q, o, m_run, l_run);
+            const int jn = (t0 == 0 && fresh && pg == new_pg) ? pos_lb % KV_PAGE_TOKENS : -1;
+            const __half* kb = stage_buf + i * 2 * PAGE_ELEMS + lane * DPL;
+            page_math<DPL>(kb, kb + PAGE_ELEMS, min(KV_PAGE_TOKENS, L - pg * KV_PAGE_TOKENS), jn, kn, vn, q, o, m_run, l_run);
         }
-        if (t0 + TILE_PAGES < my_pages) __syncthreads();   // tile buffers are re-filled by the next TMA
+        if (t0 + STAGE_PAGES < my_pages) __syncthreads();           // slots are re-filled by the next tile's copies
     }
 
+    // the two warps of a head: the second hands its partial to the first through shared memory
+    if (half == 1) {
+        if (DPL == 4) *reinterpret_cast<float4*>(&pair_o[hw][lane * DPL]) = make_float4(o[0], o[1], o[DPL - 2], o[DPL - 1]);
+        else *reinterpret_cast<float2*>(&pair_o[hw][lane * DPL]) = make_float2(o[0], o[1]);
+        if (lane == 0) { pair_ml[hw][0] = m_run; pair_ml[hw][1] = l_run; }
+    }
+    __syncthreads();
     if (tr) tr[2] = globaltimer_ns();
-    if constexpr (CL) {
-        const int G = grp * HD, slice = G / S;      // rank r merges outputs [r * slice, (r + 1) * slice) of this KV head's group
-        if (split < active) {
-            const int f = warp * HD + lane * DPL;   // this lane's dims in the group's flat output
-            const uint32_t dst = attn_mapa(smem_u32(&rx_o[split][f % slice]), (uint32_t)(f / slice));
-            if (DPL == 4) asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "f"(o[0]), "f"(o[1]), "f"(o[DPL - 2]), "f"(o[DPL - 1]) : "memory");
-            else asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(dst), "f"(o[0]), "f"(o[1]) : "memory");
-            const int per_head = HD / slice;        // ranks that hold slices of this warp's head
-            if (lane < per_head) {
-                const uint32_t dml = attn_mapa(smem_u32(&rx_ml[split][0]), (uint32_t)(warp * per_head + lane));
-                asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(dml), "f"(m_run), "f"(l_run) : "memory");
-            }
-        }
-        asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-        asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-        const int t = threadIdx.x;
-        if (t < slice) {
-            float M = -INFINITY;
-            for (int sp = 0; sp < active; ++sp) M = fmaxf(M, rx_ml[sp][0]);
-            float acc = 0.f, den = 0.f;
-            for (int sp = 0; sp < active; ++sp) {   // splits in order: deterministic
-                const float w = expf(rx_ml[sp][0] - M);
-                den += w * rx_ml[sp][1];
-                acc += w * rx_o[sp][t];
-            }
-            p.out[(size_t)kvh * G + split * slice + t] = acc / den;
-        }
-        return;
-    }
-    if (active == 1) {
-        const float inv = 1.0f / l_run;
-        float* out = p.out + (size_t)head * HD + lane * DPL;
+    if (half == 0 && split < active) {
+        const float m1 = pair_ml[hw][0], l1 = pair_ml[hw][1];
+        const float M = fmaxf(m_run, m1);                           // split < active: this split has a page, so M is finite
+        const float w0 = m_run == -INFINITY ? 0.f : expf(m_run - M), w1 = m1 == -INFINITY ? 0.f : expf(m1 - M);
 #pragma unroll
-        for (int d = 0; d < DPL; ++d) out[d] = o[d] * inv;
+        for (int d = 0; d < DPL; ++d) o[d] = o[d] * w0 + pair_o[hw][lane * DPL + d] * w1;
+        m_run = M;
+        l_run = l_run * w0 + l1 * w1;
+    }
+    if (active == 1) {                                              // one page: split 0 holds the result, no merge
+        if (split == 0 && half == 0) {
+            const float inv = 1.0f / l_run;
+            float* out = p.out + (size_t)head * HD + lane * DPL;
+#pragma unroll
+            for (int d = 0; d < DPL; ++d) out[d] = o[d] * inv;
+        }
         return;
     }
-    // partial result of (head, split)
-    {
-        float* po = p.part_o + ((size_t)head * p.n_splits + split) * HD + lane * DPL;
-        if (DPL == 4) *reinterpret_cast<float4*>(po) = make_float4(o[0], o[1], o[DPL - 2], o[DPL - 1]);
-        else *reinterpret_cast<float2*>(po) = make_float2(o[0], o[1]);
-        if (lane == 0) {
-            p.part_ml[((size_t)head * p.n_splits + split) * 2] = m_run;
-            p.part_ml[((size_t)head * p.n_splits + split) * 2 + 1] = l_run;
+    const int G = grp * HD, slice = G / S;                          // rank r merges outputs [r * slice, (r + 1) * slice) of the group
+    if (half == 0 && split < active) {
+        const int f = hw * HD + lane * DPL;                         // this lane's dims in the group's flat output
+        const uint32_t dst = attn_mapa(smem_u32(&rx_o[split][f % slice]), (uint32_t)(f / slice));
+        if (DPL == 4) asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "f"(o[0]), "f"(o[1]), "f"(o[DPL - 2]), "f"(o[DPL - 1]) : "memory");
+        else asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(dst), "f"(o[0]), "f"(o[1]) : "memory");
+        if (lane < S) {                                             // (max, sum) of this head to every rank
+            const uint32_t dml = attn_mapa(smem_u32(&rx_ml[split][hw][0]), (uint32_t)lane);
+            asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(dml), "f"(m_run), "f"(l_run) : "memory");
         }
     }
-    __syncthreads();
-    if (p.trace != nullptr && threadIdx.x == 0) atomicMax(p.trace + 5, globaltimer_ns());      // (profiling) last partial written
-    if (threadIdx.x == 0) {
-        unsigned ticket;
-        asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], 1;" : "=r"(ticket) : "l"(p.counters + kvh) : "memory");
-        if (p.trace != nullptr) atomicMax(p.trace + 6, globaltimer_ns());                           // (profiling) last ticket drawn
-        is_last = (ticket == (unsigned)active - 1);
-        if (is_last) p.counters[kvh] = 0;      // ready for the next launch
+    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+    const int t = threadIdx.x;
+    if (t < slice) {
+        const int f = split * slice + t, hh = f / HD;
+        float M = -INFINITY;
+        for (int sp = 0; sp < active; ++sp) M = fmaxf(M, rx_ml[sp][hh][0]);
+        float acc = 0.f, den = 0.f;
+        for (int sp = 0; sp < active; ++sp) {                       // splits in rank order: deterministic
+            const float w = expf(rx_ml[sp][hh][0] - M);
+            den += w * rx_ml[sp][hh][1];
+            acc += w * rx_o[sp][t];
+        }
+        p.out[(size_t)kvh * G + f] = acc / den;
     }
-    __syncthreads();
-    if (!is_last) return;
-    attn_merge_head<DPL, 32>(p.part_o, p.part_ml, p.out, head, p.n_splits, active, lane);      // all 32 partials in one round trip
-    if (p.trace != nullptr && lane == 0) atomicMax(p.trace + 7, globaltimer_ns());                  // (profiling) last merge done
+    if (tr) tr[3] = globaltimer_ns();
 }
+
+size_t attn_stage_bytes(int head_dim) { return (size_t)STAGE_PAGES * 2 * KV_PAGE_TOKENS * head_dim * sizeof(__half); }
 
 }  // namespace
 
-// cluster mode needs: 8 or 16 splits (16 = a non-portable cluster size), and a slice of the group's output per rank that lies
-// inside one head and is at least one lane's dims wide
-bool attn_cluster_ok(int n_head, int n_kv_heads, int head_dim, int n_splits) {
-    if (n_kv_heads < 1 || n_head % n_kv_heads || (n_splits != 8 && n_splits != 16)) return false;
+// 8 or 16 splits (16 = a non-portable cluster size), and a slice of the group's output per rank that is a whole number of
+// lanes' dims and fits the receive buffer
+bool attn_splits_ok(int n_head, int n_kv_heads, int head_dim, int n_splits) {
+    if (n_kv_heads < 1 || n_head % n_kv_heads || (n_splits != 8 && n_splits != 16) || (head_dim != 64 && head_dim != 128)) return false;
     const int grp = n_head / n_kv_heads, G = grp * head_dim;
     if (grp > MAX_GRP || G % n_splits) return false;
-    const int slice = G / n_splits, dpl = head_dim / 32;
-    return slice <= head_dim && head_dim % slice == 0 && slice % dpl == 0 && slice <= 32 * grp && slice <= 128;
+    const int slice = G / n_splits;
+    return slice % (head_dim / 32) == 0 && slice <= 128;
 }
 
 cudaError_t attn_decode_configure() {
-    cudaError_t e = cudaFuncSetAttribute(attn_decode_kernel<4, true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_decode_kernel<2, true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    cudaError_t e = cudaFuncSetAttribute(attn_decode_kernel<4>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_decode_kernel<2>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_decode_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_stage_bytes(128));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_decode_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_stage_bytes(64));
     return e;
 }
 
 cudaError_t attn_decode_launch(const AttnParams& p, bool pdl, cudaStream_t s) {
+    if (!attn_splits_ok(p.n_head, p.n_kv_heads, p.head_dim, p.n_splits)) return cudaErrorInvalidValue;
     const int grp = p.n_head / p.n_kv_heads;
-    if (grp < 1 || grp > MAX_GRP || p.n_head % p.n_kv_heads || p.n_splits < 1 || p.n_splits > 32) return cudaErrorInvalidValue;
-    if (p.cluster && !attn_cluster_ok(p.n_head, p.n_kv_heads, p.head_dim, p.n_splits)) return cudaErrorInvalidValue;
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3((unsigned)p.n_kv_heads, (unsigned)p.n_splits);
-    cfg.blockDim = dim3(32u * grp);
-    cfg.dynamicSmemBytes = 0;
+    cfg.blockDim = dim3(32u * WPH * grp);
+    cfg.dynamicSmemBytes = attn_stage_bytes(p.head_dim);
     cfg.stream = s;
     cudaLaunchAttribute at[2];
     int na = 0;
@@ -241,21 +270,12 @@ cudaError_t attn_decode_launch(const AttnParams& p, bool pdl, cudaStream_t s) {
         at[na].val.programmaticStreamSerializationAllowed = 1;
         ++na;
     }
-    if (p.cluster) {
-        at[na].id = cudaLaunchAttributeClusterDimension;
-        at[na].val.clusterDim.x = 1; at[na].val.clusterDim.y = (unsigned)p.n_splits; at[na].val.clusterDim.z = 1;
-        ++na;
-    }
+    at[na].id = cudaLaunchAttributeClusterDimension;
+    at[na].val.clusterDim.x = 1; at[na].val.clusterDim.y = (unsigned)p.n_splits; at[na].val.clusterDim.z = 1;
+    ++na;
     cfg.attrs = at;
     cfg.numAttrs = na;
-    if (p.cluster) {
-        if (p.head_dim == 128) return cudaLaunchKernelEx(&cfg, attn_decode_kernel<4, true>, p);
-        if (p.head_dim == 64) return cudaLaunchKernelEx(&cfg, attn_decode_kernel<2, true>, p);
-        return cudaErrorInvalidValue;
-    }
-    if (p.head_dim == 128) return cudaLaunchKernelEx(&cfg, attn_decode_kernel<4, false>, p);
-    if (p.head_dim == 64) return cudaLaunchKernelEx(&cfg, attn_decode_kernel<2, false>, p);
-    return cudaErrorInvalidValue;
+    return p.head_dim == 128 ? cudaLaunchKernelEx(&cfg, attn_decode_kernel<4>, p) : cudaLaunchKernelEx(&cfg, attn_decode_kernel<2>, p);
 }
 
 }  // namespace gl

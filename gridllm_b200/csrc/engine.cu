@@ -182,9 +182,7 @@ Status Engine::load(const std::string& path, int device, const gl_engine_opts* o
     polite_tracks_ = std::max(0, env_int("GL_POLITE_TRACKS", 3));
     sampler_pdl_ = env_int("GL_SAMPLER_PDL", 0) != 0;
     greedy_pdl_ = env_int("GL_GREEDY_PDL", 0) != 0;
-    attn_splits_ = std::max(1, std::min(32, env_int("GL_ATTN_SPLITS", 32)));
-    attn_cluster_ = env_int("GL_ATTN_CLUSTER", 0) != 0;      // the splits of a KV head as one thread-block cluster (attention.cu); needs 8 / 16 splits
-    if (attn_cluster_ && attn_splits_ != 8 && attn_splits_ != 16) attn_splits_ = 16;
+    attn_splits_ = env_int("GL_ATTN_SPLITS", 16) == 8 ? 8 : 16;      // the splits of a KV head = one thread-block cluster (attention.cu)
     prefill_mode_ = env_int("GL_PREFILL", opts ? opts->prefill_mode : 0);
     prefill_min_ = env_int("GL_PREFILL_MIN", 8);
     prefill_tc5_ = env_int("GL_PREFILL_TC5", 1) != 0;
@@ -242,7 +240,7 @@ Status Engine::load(const std::string& path, int device, const gl_engine_opts* o
     CU(gemm_tc5_configure());
     CU(flash_prefill_configure());
     CU(attn_decode_configure());
-    if (attn_cluster_ && !attn_cluster_ok(n_head_, n_kv_, hd_, attn_splits_)) attn_cluster_ = false;      // shapes the slices do not fit: the ticket path
+    if (!attn_splits_ok(n_head_, n_kv_, hd_, attn_splits_)) return fail(GL_ERR_UNSUPPORTED, "decode attention: no cluster split of this head layout");
 
     // ---- weights -> HBM -------------------------------------------------------------------------
     ST(upload_matrix(*te, tok_embd_, /*native=*/true));
@@ -603,9 +601,7 @@ Status Engine::enqueue_step(cudaStream_t s, bool with_head, bool keep_logits, in
         {
             AttnParams a{};
             a.q = q_; a.k_cache = kc; a.v_cache = vc; a.page_table = page_table_; a.n_table = n_pages_; a.st = st_; a.out = attn_;
-            a.part_o = part_o_; a.part_ml = part_ml_; a.counters = counters_;
             a.n_head = n_head_; a.n_kv_heads = n_kv_; a.head_dim = hd_; a.n_splits = attn_splits_; a.scale = scale;
-            a.cluster = attn_cluster_ ? 1 : 0;
             a.trace = perop_trace_ ? perop_trace_ + 16 * (size_t)std::min(*n_launch, PEROP_TRACE_LAUNCHES - 1) : nullptr;
             CU(attn_decode_launch(a, pdl && fused_, s));
             ++*n_launch;

@@ -169,7 +169,6 @@ private:
     bool lean_rings_ = true;   // one ring slot per warp for single-round kernels (room for the next kernel's CTAs)
     bool use_graph_ = true, use_pdl_ = true, fused_ = true;
     int smem_kb_ = 224, attn_splits_ = 16;
-    bool attn_cluster_ = false;
     int prefill_mode_ = 0, prefill_min_ = 8;
     bool have_w16_ = false, prefill_bf16_ = false, prefill_tc5_ = true;
     bool prefill_fuse_rope_ = true;  // RoPE / split / cache append in the QKV GEMM's epilogue (GL_PREFILL_FUSE_ROPE=0: the stand-alone kernel)

@@ -112,17 +112,14 @@ struct AttnParams {
     int n_table;            // entries in page_table
     const StepState* st;    // attends to positions 0..st->pos
     float* out;             // [n_head][head_dim]
-    float* part_o;          // [n_head][n_splits][head_dim]
-    float* part_ml;         // [n_head][n_splits][2]
-    unsigned* counters;     // [n_kv_heads], zero between launches
-    int n_head, n_kv_heads, head_dim, n_splits;
+    int n_head, n_kv_heads, head_dim;
+    int n_splits;           // 8 or 16: the CTAs of one KV head, one thread-block cluster (attn_splits_ok)
     float scale;
     unsigned long long* trace;   // optional (GL_TRACE=1): [2 CTAs][8] %globaltimer stamps
-    int cluster;            // 1: the splits of a KV head form one thread-block cluster and merge through distributed shared memory
 };
 cudaError_t attn_decode_launch(const AttnParams& p, bool pdl, cudaStream_t s);
 cudaError_t attn_decode_configure();
-bool attn_cluster_ok(int n_head, int n_kv_heads, int head_dim, int n_splits);
+bool attn_splits_ok(int n_head, int n_kv_heads, int head_dim, int n_splits);
 
 struct SampleParams {
     const float* logits;

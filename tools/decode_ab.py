@@ -1,5 +1,5 @@
 """Batch-1 decode A/B on the GPU box: ms per token of the Llama-3-8B-shaped q4_K_M model at ctx 1 / 576 / 2000 under a list of
-switch settings (DECODE_VARIANTS="GL_NONE=1;GL_ATTN_CLUSTER=1,GL_ATTN_SPLITS=8;..."), CUDA events around graph replays
+switch settings (DECODE_VARIANTS="GL_NONE=1;GL_ATTN_SPLITS=8;..."), CUDA events around graph replays
 (gl_time_decode).  The roofline fraction is algorithmic weight bytes / time / the measured HBM peak."""
 import json
 import os

@@ -67,8 +67,8 @@ def main():
         print(f'{name:8s} {np.mean(r[:, 4] - r[:, 1]):7.0f} {np.mean(r[:, 5] - r[:, 4]):7.0f} {np.mean(r[:, 2] - r[:, 5]):7.0f}')
     r = np.array([t8[1 + 5 * il + 1][0] for il in range(32)], dtype=np.float64)
     o = np.array([t8[1 + 5 * il + 2][0] for il in range(32)], dtype=np.float64)
-    print('ATTN tail, mean ns after the upstream wait (first CTA): math done %.0f | last partial %.0f | last ticket %.0f | last merge %.0f | attn_output wait over %.0f'
-          % (np.mean(r[:, 2] - r[:, 1]), np.mean(r[:, 5] - r[:, 1]), np.mean(r[:, 6] - r[:, 1]), np.mean(r[:, 7] - r[:, 1]), np.mean(o[:, 1] - r[:, 1])))
+    print('ATTN tail, mean ns after the upstream wait (first CTA): pages done %.0f | merged %.0f | attn_output wait over %.0f'
+          % (np.mean(r[:, 2] - r[:, 1]), np.mean(r[:, 3] - r[:, 1]), np.mean(o[:, 1] - r[:, 1])))
     # one layer in detail
     il = 16
     base = None
