@@ -55,6 +55,8 @@ static_assert(offsetof(gl_sample_opts, format) == 64, "format sits where reserve
 static_assert(sizeof(gl_engine_opts) == 64, "gl_engine_opts size is part of the ABI");
 static_assert(offsetof(gl_engine_opts, batch_weights) == 28 && offsetof(gl_engine_opts, prefix_cache) == 32 &&
                   offsetof(gl_engine_opts, reserved) == 36, "prefix_cache sits where reserved[0] was");
+// batch_prefix_cache is the first of the remaining reserved words (gl_engine_opts.reserved[GL_OPT_BATCH_PREFIX_CACHE]), at offset 36
+static_assert(GL_OPT_BATCH_PREFIX_CACHE == 0 && sizeof(gl_engine_opts) == 64, "batch_prefix_cache sits in reserved[0]");
 
 // the format field of a generating request; nullptr when valid
 const char* check_format(const gl_sample_opts& so) {

@@ -189,6 +189,7 @@ Status Engine::load(const std::string& path, int device, const gl_engine_opts* o
     prefill_flash_ = env_int("GL_PREFILL_FLASH", 1) != 0;
     prefill_fuse_rope_ = env_int("GL_PREFILL_FUSE_ROPE", 1) != 0;
     prefix_cache_ = opts && opts->prefix_cache != 0;
+    batch_prefix_cache_ = opts && opts->reserved[GL_OPT_BATCH_PREFIX_CACHE] != 0;
 
     std::string err = gguf_.open(path);
     if (!err.empty()) return fail(err.find("cannot open") == 0 ? GL_ERR_IO : GL_ERR_FORMAT, err);
@@ -334,8 +335,7 @@ Status Engine::load(const std::string& path, int device, const gl_engine_opts* o
     CU(dalloc((void**)&out_ids_, (size_t)max_out_ * 4));
     CU(dalloc((void**)&out_lp_, (size_t)max_out_ * 4));
     // physical pages are handed out in reverse order so that the page table is a real indirection
-    free_pages_.resize(pool_pages_);
-    for (int i = 0; i < pool_pages_; ++i) free_pages_[i] = i;
+    pages_.init(pool_pages_);
 
     // RoPE tables (oracle/llama_oracle.py rope_table): inv_freq rounded to fp32, angle formed in fp32,
     // cos/sin evaluated in double, rounded to fp32.
@@ -411,7 +411,7 @@ const DevMatrix* Engine::find_matrix(const std::string& name) const {
 // KV pages
 // -------------------------------------------------------------------------------------------------
 Status Engine::kv_reset() {
-    for (int p : seq_pages_) free_pages_.push_back(p);
+    for (int p : seq_pages_) pages_.release(p);
     seq_pages_.clear();
     cached_ids_.clear();
     host_pos_ = 0;
@@ -422,10 +422,8 @@ Status Engine::ensure_pages(int n_tokens) {
     if (n_tokens > n_ctx_) return fail(GL_ERR_CONTEXT, "sequence of " + std::to_string(n_tokens) + " tokens exceeds the engine context " + std::to_string(n_ctx_));
     const int need = (n_tokens + KV_PAGE_TOKENS - 1) / KV_PAGE_TOKENS;
     bool grew = false;
-    while ((int)seq_pages_.size() < need) {
-        if (free_pages_.empty()) return fail(GL_ERR_NOMEM, "KV page pool exhausted");
-        seq_pages_.push_back(free_pages_.back());
-        free_pages_.pop_back();
+    while ((int)seq_pages_.size() < need) {      // free pages first, then retained prefix pages of closed batch slots
+        if (!pages_.alloc(1, seq_pages_)) return fail(GL_ERR_NOMEM, "KV page pool exhausted");
         grew = true;
     }
     if (grew) CU(cudaMemcpyAsync(page_table_, seq_pages_.data(), seq_pages_.size() * 4, cudaMemcpyHostToDevice, stream_));

@@ -17,6 +17,7 @@
 #include "batch.h"
 #include "qgemm.h"
 #include "decode_mega.h"
+#include "prefix_pages.h"
 #include "tokenizer.h"
 
 namespace gl {
@@ -76,7 +77,6 @@ public:
     Status seq_stats(int slot, gl_gen_stats* out) const;
     void batch_counters(uint64_t out[8], bool reset) {
         for (int i = 0; i < 8; ++i) { out[i] = bc_[i]; if (reset) bc_[i] = 0; }
-        out[7] = have_qg_ ? 2 : 1;                    // which weights the batched step reads (2: quantised, 1: 16-bit copy)
     }
     Status time_batch_step(int batch, int ctx_len, int iters, float* ms, int* launches, uint64_t* wbytes);
     Status sample_logits(const float* logits, int n_vocab, const gl_sample_opts& so, int out_index, int* id, float* logprob);
@@ -124,9 +124,10 @@ private:
     Status prefill_chunk(int pos0, int n, int* n_launch);
     static constexpr int PF_CHUNK = 4096;             // rows of one prompt pass (the prefill scratch never grows past it)
     // embeddings: several sequences in ONE prompt pass (block-diagonal causal attention); seq s = rows [starts[s], starts[s] + lens[s])
-    // tables: per sequence, the device page table its K / V rows are cached through (null: nothing is cached -- embeddings)
+    // tables: per sequence, the device page table its K / V rows are cached through (null: nothing is cached -- embeddings);
+    // pos0: per sequence, the absolute position of its first row (null: all 0), earlier positions being in its pages already
     Status prefill_packed(const std::vector<int>& starts, const std::vector<int>& lens, int t_rows, int* n_launch,
-                          const std::vector<const int*>* tables = nullptr);
+                          const std::vector<const int*>* tables = nullptr, const std::vector<int>* pos0 = nullptr);
     static constexpr int EMB_PACK_TOKENS = 2048;      // rows of one packed pass (each sequence starts on a 128-row boundary)
     int* pk_ids_ = nullptr;                           // [EMB_PACK_TOKENS] token ids of a pack (pad rows: token 0)
     float *emb_out_ = nullptr, *emb_rstd_ = nullptr, *emb_pooled_ = nullptr;
@@ -209,7 +210,7 @@ private:
     int n_pages_ = 0;                                // entries of ONE sequence's page table (n_ctx / 16)
     int pool_pages_ = 0;                             // physical pages of the pool all sequences share
     int* page_table_ = nullptr;                      // device
-    std::vector<int> free_pages_;
+    PagePool pages_;                                 // every physical page: free, referenced or retained (prefix_pages.h)
     std::vector<int> seq_pages_;
     StepState* st_ = nullptr;
     int* prompt_ids_ = nullptr;
@@ -225,8 +226,9 @@ private:
     // ---- continuous batching (engine_batch.cu) ----
     struct SeqSlot {
         bool open = false, done = false, first_pending = false;
-        std::vector<int> pages;
+        std::vector<int> pages;                       // its page table: the shared prefix pages, then its own
         int n_prompt = 0, n_pred = 0, produced = 0;
+        int n_shared = 0;                             // prompt positions [0, n_shared) read from shared pages (not evaluated)
         DrawPlan plan;
         int32_t last_token = 0;
         float first_lp = 0.f;
@@ -277,6 +279,17 @@ private:
     Status check_pre_draw(int variant);
     Status ensure_batch_penalty();                    // bprompt_ / bpen_counts_, allocated when the first penalised sequence opens
     Status keep_prompt(int slot, const int32_t* prompt, int n_prompt);     // a penalised slot's prompt -> bprompt_
+    // prompt-prefix sharing between slots (gl_engine_opts batch_prefix_cache; prefix_pages.h): on when the option is and the
+    // prompt pass can start past a shared prefix (fused prompt attention, not the persistent decode kernel)
+    bool batch_prefix_cache_ = false;
+    bool share_prefixes() const { return batch_prefix_cache_ && prefill_flash_ && !use_mega_; }
+    // a slot's table for `prompt`: the indexed pages of the longest matching chain, cut by the reuse rule (referenced), then
+    // pages of its own for the rest of n_prompt + n_pred tokens; *r = positions taken from the shared pages.  false (nothing
+    // held) when the pool cannot supply the own pages.
+    bool take_pages(const int32_t* prompt, int n_prompt, int n_pred, bool share, std::vector<int>* pages, int* r);
+    void release_pages(std::vector<int>& pages);
+    // index the prompt-pass pages [0, n_prompt / 16) of a table, from page `from` on; the pages it added go to *added
+    void index_prompt_pages(const int32_t* prompt, int n_prompt, const std::vector<int>& pages, int from, std::vector<int>* added);
     static int bucket_of(int rows) { int b = 8; while (b < rows) b <<= 1; return b; }
     static int bucket_index(int bucket) { int i = 0; while ((8 << i) < bucket) ++i; return i; }
 

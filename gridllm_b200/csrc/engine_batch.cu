@@ -207,6 +207,36 @@ Status Engine::keep_prompt(int slot, const int32_t* prompt, int n_prompt) {
     return {};
 }
 
+bool Engine::take_pages(const int32_t* prompt, int n_prompt, int n_pred, bool share, std::vector<int>* pages, int* r) {
+    pages->clear();
+    *r = 0;
+    if (share) {
+        const int l = pages_.match(prompt, n_prompt, pages);
+        *r = shared_prefix_reuse(l, n_prompt, prefill_min_);
+        pages->resize(*r / KV_PAGE_TOKENS);
+        for (int p : *pages) pages_.ref(p);            // before the allocation below, which may evict retained pages
+    }
+    const int own = (n_prompt + n_pred + KV_PAGE_TOKENS - 1) / KV_PAGE_TOKENS - *r / KV_PAGE_TOKENS;
+    if (!pages_.alloc(own, *pages)) {
+        release_pages(*pages);
+        *r = 0;
+        return false;
+    }
+    return true;
+}
+
+void Engine::release_pages(std::vector<int>& pages) {
+    for (int p : pages) pages_.release(p);
+    pages.clear();
+}
+
+void Engine::index_prompt_pages(const int32_t* prompt, int n_prompt, const std::vector<int>& pages, int from, std::vector<int>* added) {
+    for (int j = from; j < n_prompt / KV_PAGE_TOKENS; ++j) {
+        if (!pages_.insert(j > 0 ? pages[j - 1] : -1, prompt + (size_t)j * KV_PAGE_TOKENS, pages[j])) break;      // already indexed
+        if (added) added->push_back(pages[j]);
+    }
+}
+
 // Prefill a prompt into a free slot's own pages and draw its first token.  The single-sequence code runs unchanged on the
 // slot's state: the members it reads (page table, step state, output buffers) point at the slot's rows for the duration.
 // One prompt.  It takes the SAME path as a prompt opened together with others (gl_seq_open_many with one entry: packed prompt
@@ -239,17 +269,19 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
     for (int i = 0; i < max_batch_; ++i)
         if (!slots_[i].open) { slot = i; break; }
     if (slot < 0) return failb(GL_ERR_NOMEM, "no free sequence slot (max_batch " + std::to_string(max_batch_) + ")");
-    const int need = (n_prompt + n_pred + KV_PAGE_TOKENS - 1) / KV_PAGE_TOKENS;      // reserved up front: a step can never run out
-    if ((int)free_pages_.size() < need) return failb(GL_ERR_NOMEM, "KV page pool exhausted");
+    // pages for every position it will hold, reserved up front: a step can never run out.  Only a prompt that takes the prompt
+    // pass shares a prefix (and indexes its pages afterwards); short prompts step through the decode kernels.
+    const bool share = share_prefixes() && can_batch_prefill(0, n_prompt);
     SeqSlot& S = slots_[slot];
     S = SeqSlot{};
-    for (int i = 0; i < need; ++i) { S.pages.push_back(free_pages_.back()); free_pages_.pop_back(); }
+    int r = 0;
+    if (!take_pages(prompt, n_prompt, n_pred, share, &S.pages, &r)) return failb(GL_ERR_NOMEM, "KV page pool exhausted");
     int* table = btables_ + (size_t)slot * n_pages_;
     CU(cudaMemcpyAsync(table, S.pages.data(), S.pages.size() * 4, cudaMemcpyHostToDevice, stream_));
     if (plan.penalised) {                                 // the head of the history the batched steps penalise with
         Status ks = keep_prompt(slot, prompt, n_prompt);
         if (!ks.ok()) {
-            for (int p : S.pages) free_pages_.push_back(p);
+            release_pages(S.pages);
             S = SeqSlot{};
             return ks;
         }
@@ -267,7 +299,7 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
         if (ce != cudaSuccess) { rs = failb(GL_ERR_CUDA, cudaGetErrorString(ce)); break; }
         if (can_batch_prefill(0, n_prompt)) {      // any length: passes of PF_CHUNK rows, the later ones over the slot's pages
             rs = set_state(n_prompt - 1, prompt[n_prompt - 1], n_prompt, 0, &so, plan);
-            if (rs.ok()) rs = prefill_batched(0, n_prompt, &dummy);
+            if (rs.ok()) rs = prefill_batched(r, n_prompt - r, &dummy);      // positions [0, r) are in the shared pages
             if (rs.ok()) rs = enqueue_head(stream_, false, &dummy);
         } else {      // short prompts: plain launches of the decode step (the captured graphs hold the engine's own pointers)
             rs = set_state(0, prompt[0], n_prompt, 0, &so, plan);
@@ -291,14 +323,17 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
     } while (false);
     page_table_ = sv.pt; st_ = sv.st; out_ids_ = sv.oi; out_lp_ = sv.ol; host_pos_ = sv.hp;
     if (!rs.ok()) {
-        for (int p : S.pages) free_pages_.push_back(p);
+        release_pages(S.pages);
         S = SeqSlot{};
         return rs;
     }
+    if (share) index_prompt_pages(prompt, n_prompt, S.pages, r / KV_PAGE_TOKENS, nullptr);
     S.open = true;
+    S.n_shared = r;
     S.n_prompt = n_prompt; S.n_pred = n_pred; S.produced = 0; S.plan = plan; S.first_pending = true;
     S.t_open_ns = t_open; S.launches = prefill_launches; S.stopped = S.done;
-    bc_[3] += (uint64_t)S.prefill_ns; bc_[4] += (uint64_t)n_prompt; bc_[5] += 1; bc_[6] += (uint64_t)prefill_launches;
+    bc_[3] += (uint64_t)S.prefill_ns; bc_[4] += (uint64_t)(n_prompt - r); bc_[5] += 1; bc_[6] += (uint64_t)prefill_launches;
+    bc_[7] += (uint64_t)r;
     *slot_out = slot;
     return {};
 }
@@ -335,34 +370,44 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
         CU(dalloc((void**)&emb_rstd_, (size_t)std::max(EMB_PACK_TOKENS, n_ctx_) * 4));
     }
     const bool packable = have_w16_ && prefill_mode_ != 1;
+    const bool share = packable && share_prefixes();
     const int64_t t_open = std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now().time_since_epoch()).count();
     int next = 0;
     std::vector<int32_t> h_ids(EMB_PACK_TOKENS);
     while (next < n_seq) {
         // ---- one pack: as many of the next prompts as fit EMB_PACK_TOKENS rows, free slots and free pages ----
-        std::vector<int> starts, lens, which, pslots;
+        std::vector<int> starts, lens, which, pslots, shared;
         std::vector<const int*> tables;
+        std::vector<int> indexed;                    // pages this pack added to the prefix index (taken out again if its pass fails)
         int rows = 0;
         bool out_of_room = false;
         std::fill(h_ids.begin(), h_ids.end(), 0);
         while (next < n_seq && (int)which.size() < MAX_BATCH) {
-            const int n = offs[next + 1] - offs[next], lp = (n + 127) / 128 * 128;
+            const int32_t* prompt = ids + offs[next];
+            const int n = offs[next + 1] - offs[next];
             if (!packable || n > EMB_PACK_TOKENS || n < prefill_min_) break;              // this one goes through gl_seq_open's own path
-            if (rows + lp > EMB_PACK_TOKENS) break;
+            // the positions a shared prefix covers are not evaluated: only the suffix takes rows of the pack
+            const int r_max = share ? shared_prefix_reuse(pages_.match(prompt, n, nullptr), n, prefill_min_) : 0;
+            if (rows + (n - r_max + 127) / 128 * 128 > EMB_PACK_TOKENS) break;
             const int n_pred = opts[next].num_predict > 0 ? opts[next].num_predict : 128;
-            const int need = (n + n_pred + KV_PAGE_TOKENS - 1) / KV_PAGE_TOKENS;
             int slot = -1;
             for (int k = 0; k < max_batch_; ++k)
                 if (!slots_[k].open && std::find(pslots.begin(), pslots.end(), k) == pslots.end()) { slot = k; break; }
-            if (slot < 0 || (int)free_pages_.size() < need) { out_of_room = true; break; }
+            if (slot < 0) { out_of_room = true; break; }
             SeqSlot& S = slots_[slot];
             S = SeqSlot{};
-            for (int k = 0; k < need; ++k) { S.pages.push_back(free_pages_.back()); free_pages_.pop_back(); }
+            int r = 0;
+            if (!take_pages(prompt, n, n_pred, share, &S.pages, &r)) { out_of_room = true; break; }
             CU(cudaMemcpyAsync(btables_ + (size_t)slot * n_pages_, S.pages.data(), S.pages.size() * 4, cudaMemcpyHostToDevice, stream_));
-            std::memcpy(h_ids.data() + rows, ids + offs[next], (size_t)n * 4);
-            starts.push_back(rows); lens.push_back(n); which.push_back(next); pslots.push_back(slot);
+            // its prompt pages go into the index now, so that later prompts of this pack share them: the QKV projection of every
+            // layer writes this sequence's K / V rows to its pages before that layer's attention reads them through a sharer's
+            // table (a sharer comes after its owner in the pack)
+            if (share) index_prompt_pages(prompt, n, S.pages, r / KV_PAGE_TOKENS, &indexed);
+            const int len = n - r;
+            std::memcpy(h_ids.data() + rows, prompt + r, (size_t)len * 4);
+            starts.push_back(rows); lens.push_back(len); which.push_back(next); pslots.push_back(slot); shared.push_back(r);
             tables.push_back(btables_ + (size_t)slot * n_pages_);
-            rows += lp;
+            rows += (len + 127) / 128 * 128;
             ++next;
         }
         if (which.empty()) {
@@ -388,7 +433,7 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             cudaError_t ce = cudaMemcpyAsync(pk_ids_, h_ids.data(), (size_t)rows * 4, cudaMemcpyHostToDevice, stream_);
             if (ce == cudaSuccess) ce = cudaEventRecord(ev_[2], stream_);
             if (ce != cudaSuccess) { rs = failb(GL_ERR_CUDA, cudaGetErrorString(ce)); break; }
-            rs = prefill_packed(starts, lens, rows, &launches, &tables);
+            rs = prefill_packed(starts, lens, rows, &launches, &tables, &shared);
             if (!rs.ok()) break;
             // first tokens: last hidden row of each sequence -> rows 0..P-1 of the batched-step buffers -> final norm -> lm_head GEMM
             for (int i = 0; i < P && ce == cudaSuccess; ++i)
@@ -408,7 +453,7 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             hc.n_rows = P;
             bool any_pen = false, any_mask = false;
             for (int i = 0; i < P && ce == cudaSuccess; ++i) {
-                const int w = which[i], n = lens[i];
+                const int w = which[i], n = lens[i] + shared[i];
                 const DrawPlan& plan = plans[w];
                 hst[i] = make_state(n - 1, ids[offs[w] + n - 1], n, 0, &opts[w]);
                 slots_[pslots[i]].plan = plan;
@@ -451,8 +496,9 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             launches += 3;
         } while (false);
         if (!rs.ok()) {
+            for (size_t k = indexed.size(); k-- > 0;) pages_.forget(indexed[k]);
             for (int i = 0; i < P; ++i) {
-                for (int p : slots_[pslots[i]].pages) free_pages_.push_back(p);
+                release_pages(slots_[pslots[i]].pages);
                 slots_[pslots[i]] = SeqSlot{};
             }
             if (*n_opened > 0) break;                // earlier packs are open and reported; the caller sees -1 for the rest
@@ -464,7 +510,8 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             SeqSlot& S = slots_[pslots[i]];
             const int w = which[i];
             S.open = true;
-            S.n_prompt = lens[i];
+            S.n_prompt = lens[i] + shared[i];
+            S.n_shared = shared[i];
             S.n_pred = opts[w].num_predict > 0 ? opts[w].num_predict : 128;
             S.produced = 0;
             S.first_pending = true;
@@ -478,6 +525,7 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             slots_out[w] = pslots[i];
             bc_[4] += (uint64_t)lens[i];
             bc_[5] += 1;
+            bc_[7] += (uint64_t)shared[i];
         }
         bc_[3] += (uint64_t)(pack_ms * 1e6);
         bc_[6] += (uint64_t)launches;
@@ -490,7 +538,7 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
 
 Status Engine::seq_close(int slot) {
     if (slot < 0 || slot >= (int)slots_.size() || !slots_[slot].open) return failb(GL_ERR_INVALID, "seq_close: no such open sequence");
-    for (int p : slots_[slot].pages) free_pages_.push_back(p);
+    release_pages(slots_[slot].pages);           // indexed prompt pages stay retained for later prompts
     slots_[slot] = SeqSlot{};
     return {};
 }
@@ -499,7 +547,7 @@ Status Engine::seq_stats(int slot, gl_gen_stats* out) const {
     if (slot < 0 || slot >= (int)slots_.size() || !slots_[slot].open || !out) return failb(GL_ERR_INVALID, "seq_stats: no such open sequence");
     const SeqSlot& S = slots_[slot];
     std::memset(out, 0, sizeof(*out));
-    out->prompt_eval_count = S.n_prompt;
+    out->prompt_eval_count = S.n_prompt - S.n_shared;      // the evaluated tokens
     out->eval_count = S.produced;
     out->prompt_eval_duration_ns = S.prefill_ns;
     out->eval_duration_ns = S.eval_ns;
@@ -763,14 +811,14 @@ Status Engine::time_batch_step(int batch, int ctx_len, int iters, float* ms, int
     const int need_tokens = ctx_len + iters + 8;
     if (need_tokens > n_ctx_) return failb(GL_ERR_CONTEXT, "time_batch_step: context too long for this engine");
     const int need = (need_tokens + KV_PAGE_TOKENS - 1) / KV_PAGE_TOKENS;
-    if ((size_t)need * batch > free_pages_.size()) return failb(GL_ERR_NOMEM, "time_batch_step: KV page pool too small for this batch");
+    if ((size_t)need * batch > (size_t)pages_.available()) return failb(GL_ERR_NOMEM, "time_batch_step: KV page pool too small for this batch");
     std::vector<StepState> hst(batch);
     std::vector<int> rows(batch);
     for (int b = 0; b < batch; ++b) {
         SeqSlot& S = slots_[b];
         S = SeqSlot{};
         S.open = true;
-        for (int i = 0; i < need; ++i) { S.pages.push_back(free_pages_.back()); free_pages_.pop_back(); }
+        pages_.alloc(need, S.pages);                 // never indexed: the pages go back to the free list
         CU(cudaMemcpyAsync(btables_ + (size_t)b * n_pages_, S.pages.data(), S.pages.size() * 4, cudaMemcpyHostToDevice, stream_));
         StepState h{};
         h.pos = ctx_len - 1; h.token = (7 + 13 * b) % n_vocab_; h.ignore_eos = 1; h.top_p = 1.f;
@@ -798,7 +846,7 @@ Status Engine::time_batch_step(int batch, int ctx_len, int iters, float* ms, int
     }
     cudaStreamSynchronize(stream_);
     for (int b = 0; b < batch; ++b) {
-        for (int p : slots_[b].pages) free_pages_.push_back(p);
+        release_pages(slots_[b].pages);
         slots_[b] = SeqSlot{};
     }
     last_rows_.clear();

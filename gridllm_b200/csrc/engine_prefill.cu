@@ -198,7 +198,10 @@ Status Engine::prefill_chunk(int pos0, int n, int* n_launch) {
 // themselves (block-diagonal causal attention: the three attention launches run per sequence on its own rows).  Nothing is
 // cached: an embedding has no decode phase.  Hidden states end up in pf_x_ for pooling.
 Status Engine::prefill_packed(const std::vector<int>& starts, const std::vector<int>& lens, int t_rows, int* n_launch,
-                              const std::vector<const int*>* tables) {
+                              const std::vector<const int*>* tables, const std::vector<int>* pos0) {
+    if (pos0 && !prefill_flash_)
+        for (int p : *pos0)
+            if (p > 0) return failp(GL_ERR_UNSUPPORTED, "a prompt pass from a non-zero position needs the fused prompt attention");
     const int TP = (t_rows + 127) / 128 * 128;
     const int qd = n_head_ * hd_, kvd = n_kv_ * hd_, ldq = qd + 2 * kvd, grp = n_head_ / n_kv_;
     ST(ensure_prefill_scratch(std::max(TP, 128)));
@@ -229,6 +232,7 @@ Status Engine::prefill_packed(const std::vector<int>& starts, const std::vector<
                     ra.segs.start[i] = starts[i];
                     ra.segs.len[i] = lens[i];
                     ra.segs.table[i] = tables ? (*tables)[i] : nullptr;
+                    ra.segs.pos0[i] = pos0 ? (*pos0)[i] : 0;
                 }
                 GemmParams gr = g;
                 gr.epi = GEMM_EPI_ROPE_SPLIT; gr.rope = &ra;
@@ -246,6 +250,7 @@ Status Engine::prefill_packed(const std::vector<int>& starts, const std::vector<
                     segs.start[i] = starts[c0 + i];
                     segs.len[i] = lens[c0 + i];
                     segs.table[i] = tables ? (*tables)[c0 + i] : nullptr;
+                    segs.pos0[i] = pos0 ? (*pos0)[c0 + i] : 0;
                     row_hi = std::max(row_hi, segs.start[i] + (segs.len[i] + 127) / 128 * 128);
                 }
                 if (c0 + PF_MAX_SEGS >= starts.size()) row_hi = std::max(row_hi, TP);      // trailing rows of the pack are zeroed too

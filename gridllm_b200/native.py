@@ -47,6 +47,16 @@ class EngineOpts(C.Structure):
                 ("prefill_mode", C.c_int32), ("max_batch", C.c_int32), ("kv_pool_tokens", C.c_int32), ("batch_weights", C.c_int32),
                 ("prefix_cache", C.c_int32), ("reserved", C.c_int32 * 7)]
 
+    GL_OPT_BATCH_PREFIX_CACHE = 0          # include/gridllm_native.h: the reserved word that holds batch_prefix_cache
+
+    @property
+    def batch_prefix_cache(self) -> int:
+        return self.reserved[self.GL_OPT_BATCH_PREFIX_CACHE]
+
+    @batch_prefix_cache.setter
+    def batch_prefix_cache(self, v: int) -> None:
+        self.reserved[self.GL_OPT_BATCH_PREFIX_CACHE] = int(v)
+
 
 class ModelInfo(C.Structure):
     _fields_ = [("arch", C.c_char * 32), ("name", C.c_char * 96), ("quantization", C.c_char * 24),
@@ -189,7 +199,7 @@ class Engine:
 
     def __init__(self, gguf_path: str, device: int = 0, max_ctx: int = 0, act_bits: int = 16, use_graph: bool = True,
                  use_pdl: bool = True, prefill_mode: int = 0, max_batch: int = 0, kv_pool_tokens: int = 0, batch_weights: int = 0,
-                 prefix_cache: bool = False):
+                 prefix_cache: bool = False, batch_prefix_cache: bool = False):
         self._lib = load_library()
         self._h = C.c_void_p()
         o = EngineOpts()
@@ -199,6 +209,8 @@ class Engine:
         o.max_batch, o.kv_pool_tokens, o.batch_weights = int(max_batch), int(kv_pool_tokens), int(batch_weights)
         # generate() keeps the KV pages of the longest prefix it shares with the previous generate() (include/gridllm_native.h)
         o.prefix_cache = int(bool(prefix_cache))
+        # seq_open / seq_open_many sequences share the KV pages of prompt prefixes, also with closed ones (include/gridllm_native.h)
+        o.batch_prefix_cache = int(bool(batch_prefix_cache))
         _check(self._lib.gl_engine_create(gguf_path.encode(), device, C.byref(o), C.byref(self._h)))
         self.info = ModelInfo()
         _check(self._lib.gl_engine_info(self._h, C.byref(self.info)))
@@ -361,7 +373,7 @@ class Engine:
         out = (C.c_uint64 * 8)()
         _check(self._lib.gl_batch_counters(self._h, out, int(reset)))
         return {"steps": out[0], "rows": out[1], "step_ns": out[2], "prefill_ns": out[3], "prefill_tokens": out[4], "sequences": out[5],
-                "launches": out[6]}
+                "launches": out[6], "shared_tokens": out[7]}
 
     def time_batch_step(self, batch: int, ctx_len: int, iters: int = 16):
         """-> (ms per batched step, kernel launches per step, weight bytes one step reads)"""

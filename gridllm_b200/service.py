@@ -110,8 +110,10 @@ class NativeInferenceService:
         engine_kw: further Engine options, e.g. prefix_cache=True: a request keeps the KV pages of the longest prefix it shares
         with the previous request on the same engine (a multi-turn client that sends metadata.context back then pays for its
         new tokens only, as with Ollama's cached prefix), and its prompt_eval_count counts the tokens it evaluated.  Off by
-        default, like the other Ollama-behaviour switches.  With max_batch > 1 the batch runner does no reuse: each sequence
-        slot owns its own pages."""
+        default, like the other Ollama-behaviour switches.  prefix_cache covers one request at a time; with max_batch > 1 pass
+        batch_prefix_cache=True instead: the batch runner's sequences share the KV pages of prompt prefixes, with each other
+        and with sequences that have closed (a common system prompt, or a chat's earlier turns, is evaluated once), and
+        prompt_eval_count counts the tokens each one evaluated."""
         self._sampling_defaults = dict(sampling_defaults or {})
         self._penalty_defaults = dict(penalty_defaults or {})
         self._json_schema = bool(json_schema)

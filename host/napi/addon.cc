@@ -78,6 +78,12 @@ napi_value CreateEngine(napi_env env, napi_callback_info info) {
             if (napi_get_value_bool(env, v, &b) == napi_ok) o.prefix_cache = b ? 1 : 0;
             else napi_get_value_int32(env, v, &o.prefix_cache);
         }
+        if (napi_get_named_property(env, argv[2], "batchPrefixCache", &v) == napi_ok) {      // boolean (or 0 / 1)
+            bool b = false;
+            int32_t& w = o.reserved[GL_OPT_BATCH_PREFIX_CACHE];
+            if (napi_get_value_bool(env, v, &b) == napi_ok) w = b ? 1 : 0;
+            else napi_get_value_int32(env, v, &w);
+        }
     }
     o.use_graph = 1;
     o.use_pdl = 1;

@@ -27,14 +27,16 @@ export class NativeInferenceService {
 	);
 	private device = parseInt(process.env.GRIDLLM_DEVICE || "0", 10);
 	// prefixCache: a generate keeps the KV pages of the longest prefix it shares with the previous generate on the same engine
-	// (a client that sends `context` back pays for its new tokens only); off by default (include/gridllm_native.h)
-	private engineOptions: { prefixCache?: boolean };
+	// (a client that sends `context` back pays for its new tokens only); off by default (include/gridllm_native.h).
+	// batchPrefixCache: the same for an engine created with maxBatch > 1: its sequences share the KV pages of prompt prefixes,
+	// with each other and with closed ones; off by default.
+	private engineOptions: { prefixCache?: boolean; batchPrefixCache?: boolean };
 	// jsonSchema: enforce a JSON-schema `format` on the GPU (gl_format_schema); off by default: a schema asks for valid JSON of
 	// any shape, as before.  Same switch as gridllm_b200/service.py's json_schema.
 	private jsonSchema: boolean;
 
-	constructor(options: { prefixCache?: boolean; jsonSchema?: boolean } = {}) {
-		this.engineOptions = { prefixCache: !!options.prefixCache };
+	constructor(options: { prefixCache?: boolean; batchPrefixCache?: boolean; jsonSchema?: boolean } = {}) {
+		this.engineOptions = { prefixCache: !!options.prefixCache, batchPrefixCache: !!options.batchPrefixCache };
 		this.jsonSchema = !!options.jsonSchema;
 	}
 

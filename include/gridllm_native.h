@@ -69,12 +69,29 @@ typedef struct gl_engine_opts {
      * kernels wrote, and the output is then within the decode-vs-prefill tolerance of a cold call, not bit-identical.
      * The record is cleared by gl_kv_reset and by every other call that writes the single-sequence pages or step state:
      * gl_prefill, gl_decode_step, gl_embed of a sequence longer than 2 048 tokens, gl_sample_logits / gl_penalize_logits /
-     * gl_constrain_logits, gl_time_decode.  No reuse under the persistent decode kernel (GL_MEGA=1), nor for gl_seq_open
-     * sequences (each slot owns its pages).  With prefix_cache on, gl_gen_stats.prompt_eval_count of gl_generate counts the
-     * tokens this call evaluated (n_prompt - r) and prompt_eval_duration their device time. */
+     * gl_constrain_logits, gl_time_decode.  No reuse under the persistent decode kernel (GL_MEGA=1); gl_seq_open sequences
+     * share prefixes through batch_prefix_cache instead.  With prefix_cache on, gl_gen_stats.prompt_eval_count of gl_generate
+     * counts the tokens this call evaluated (n_prompt - r) and prompt_eval_duration their device time. */
     int32_t prefix_cache;
+    /* reserved[GL_OPT_BATCH_PREFIX_CACHE] is batch_prefix_cache: prompt-prefix KV pages shared between gl_seq_open /
+     * gl_seq_open_many sequences; 0 = off (every slot owns all its pages and prefills its whole prompt).  Pages are
+     * reference-counted.  After a slot's prompt pass, its full prompt pages [0, floor(n_prompt / 16)) are indexed by their ids
+     * (a trie of 16-token pages, ids compared exactly); the last partial page, rows written by decode steps, prompts that
+     * stepped through the decode kernels (shorter than the prompt pass's minimum of 8 tokens, prefill_mode 1) and
+     * gl_time_batch_step's sequences never are.  A new sequence whose prompt starts with a chain of L indexed pages reads
+     * r = 16 floor(min(16 L, n_prompt - 8) / 16) positions from those pages and evaluates only [r, n_prompt): the K / V of a
+     * prompt prefix depend on its ids alone, so it gets the bits of a cold open.  Prompts of one gl_seq_open_many call that
+     * share a prefix nothing has indexed yet share the first one's pages within the same pass.  It reserves only its own
+     * pages, ceil((n_prompt + num_predict) / 16) - r / 16; every position it writes is >= r, so shared pages are never written.
+     * When its last reference closes, an indexed page is retained, and allocation (batch slots and gl_generate alike) takes
+     * free pages first, then evicts retained pages, least recently released leaves first: GL_ERR_NOMEM comes only when open
+     * sequences hold the pool.  gl_gen_stats.prompt_eval_count of gl_seq_stats counts the evaluated tokens and
+     * prompt_eval_duration their share of the pass; gl_batch_counters out[7] counts the prompt tokens taken from shared pages.
+     * No sharing under GL_PREFILL_FLASH=0 or the persistent decode kernel (GL_MEGA=1).  The other reserved words must be 0. */
     int32_t reserved[7];
 } gl_engine_opts;
+
+#define GL_OPT_BATCH_PREFIX_CACHE 0       /* index of batch_prefix_cache in gl_engine_opts.reserved */
 
 typedef struct gl_model_info {
     char     arch[32];
@@ -198,7 +215,8 @@ int  gl_embed(gl_engine* e, const int32_t* ids, const int32_t* seq_offsets, int3
  * server/src/config/index.ts:31).  With that limit raised the worker opens one sequence per job and steps them TOGETHER:
  * one batched decode step reads the weights once for every open sequence.
  *   gl_seq_open   prefill `prompt` into a free slot's own KV pages and draw its first token (reported by the next
- *                 gl_batch_step); pages for n_prompt + num_predict tokens are reserved up front, so a step cannot run out.
+ *                 gl_batch_step); pages for n_prompt + num_predict tokens are reserved up front, so a step cannot run out
+ *                 (with batch_prefix_cache, less the prompt prefix it shares).
  *                 GL_ERR_NOMEM when no slot / not enough pages are free -- the caller may retry after a gl_seq_close.
  *   gl_batch_step one token for every open, unfinished sequence.  Entry i: slots[i], ids[i], logprobs[i], done[i].
  *                 done = 1 with id >= 0: that token was the sequence's last (num_predict reached);  done = 1 with id = -1:
@@ -231,7 +249,8 @@ int  gl_token_piece(const gl_engine* e, int32_t id, char* buf, int32_t cap, int3
 int  gl_token_text(const gl_engine* e, int32_t id, char* buf, int32_t cap, int32_t* len_out);
 /* engine-wide batching counters since creation (or the last reset): out[0] batched steps, [1] sum over steps of sequences in
  * the step, [2] device ns of those steps, [3] device ns of the prefills of gl_seq_open, [4] prompt tokens prefilled,
- * [5] sequences opened, [6] kernel launches, [7] reserved.  reset != 0 zeroes them after reading. */
+ * [5] sequences opened, [6] kernel launches, [7] prompt tokens taken from shared pages (batch_prefix_cache; [4] counts the
+ * evaluated ones).  reset != 0 zeroes them after reading. */
 int  gl_batch_counters(gl_engine* e, uint64_t out[8], int32_t reset);
 /* mean device time (ms) of one batched decode step with `batch` synthetic sequences at context length ctx_len (roofline line
  * of the batched workload); weight_bytes = bytes of weights one such step reads */
