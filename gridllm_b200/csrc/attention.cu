@@ -88,7 +88,9 @@ __global__ void __launch_bounds__(32 * WPH * MAX_GRP) attn_decode_kernel(const _
     __syncthreads();
     pdl_launch_dependents();
 
-    // The position counter only grows inside a sequence, so a value read before the wait is a lower bound pos_lb: every
+    // Within a step the position counter only grows (a context shift lowers it, but kv_shift.cu runs BETWEEN steps, launched
+    // without programmatic dependent launch and never releasing its dependants early, so no kernel of the next step starts
+    // before the lowered position is visible).  A value read before the wait is therefore a lower bound pos_lb: every
     // row below it was appended by an earlier step, whose kernels have completed, and is final.  Only rows < pos_lb are
     // requested here.  Row pos_lb is written by the upstream QKV epilogue (or, if pos_lb is stale, by an earlier step that
     // may still be running); it is read only after the wait, and used only when the position read after the wait is pos_lb.

@@ -57,6 +57,10 @@ static_assert(offsetof(gl_engine_opts, batch_weights) == 28 && offsetof(gl_engin
                   offsetof(gl_engine_opts, reserved) == 36, "prefix_cache sits where reserved[0] was");
 // batch_prefix_cache is the first of the remaining reserved words (gl_engine_opts.reserved[GL_OPT_BATCH_PREFIX_CACHE]), at offset 36
 static_assert(GL_OPT_BATCH_PREFIX_CACHE == 0 && sizeof(gl_engine_opts) == 64, "batch_prefix_cache sits in reserved[0]");
+// context_shift is reserved[GL_OPT_CONTEXT_SHIFT], at offset 40; num_keep took the tail padding of gl_sample_opts (offset 68, the
+// size unchanged), which is why the engine reads it only when context_shift is on
+static_assert(GL_OPT_CONTEXT_SHIFT == 1 && offsetof(gl_engine_opts, reserved) + 4 * GL_OPT_CONTEXT_SHIFT == 40, "context_shift sits in reserved[1]");
+static_assert(offsetof(gl_sample_opts, num_keep) == 68 && sizeof(gl_sample_opts) == 72, "num_keep sits in the tail padding");
 
 // the format field of a generating request; nullptr when valid
 const char* check_format(const gl_sample_opts& so) {

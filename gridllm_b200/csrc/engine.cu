@@ -2,6 +2,7 @@
 // construction (fused sm_90a kernels, PDL, CUDA graph) and the generate / embed drivers.
 // See engine.h / include/gridllm_native.h for the reference call sites this replaces.
 #include "engine.h"
+#include "context_shift.h"
 
 #include <algorithm>
 #include <chrono>
@@ -190,6 +191,7 @@ Status Engine::load(const std::string& path, int device, const gl_engine_opts* o
     prefill_fuse_rope_ = env_int("GL_PREFILL_FUSE_ROPE", 1) != 0;
     prefix_cache_ = opts && opts->prefix_cache != 0;
     batch_prefix_cache_ = opts && opts->reserved[GL_OPT_BATCH_PREFIX_CACHE] != 0;
+    context_shift_ = opts && opts->reserved[GL_OPT_CONTEXT_SHIFT] != 0;
 
     std::string err = gguf_.open(path);
     if (!err.empty()) return fail(err.find("cannot open") == 0 ? GL_ERR_IO : GL_ERR_FORMAT, err);
@@ -427,6 +429,31 @@ Status Engine::ensure_pages(int n_tokens) {
         grew = true;
     }
     if (grew) CU(cudaMemcpyAsync(page_table_, seq_pages_.data(), seq_pages_.size() * 4, cudaMemcpyHostToDevice, stream_));
+    return {};
+}
+
+Status Engine::shift_plan(const gl_sample_opts& so, int n_prompt, int n_pred, int* keep) {
+    if (so.num_keep < -1) return fail(GL_ERR_INVALID, "num_keep must be >= -1");
+    if (n_pred > n_ctx_) return fail(GL_ERR_CONTEXT, "num_predict " + std::to_string(n_pred) + " exceeds the engine context " + std::to_string(n_ctx_) + " (the output buffers hold that many ids)");
+    *keep = shift_keep(so.num_keep, n_prompt, n_ctx_);
+    return {};
+}
+
+Status Engine::launch_shift(const std::vector<KvShiftSeq>& seqs) {
+    if (seqs.empty()) return {};
+    if (!shift_seqs_) {
+        CU(cudaMalloc((void**)&shift_seqs_, (size_t)MAX_BATCH * sizeof(KvShiftSeq)));
+        allocs_.push_back(shift_seqs_);
+    }
+    if ((int)seqs.size() > MAX_BATCH) return fail(GL_ERR_INVALID, "kv_shift: too many sequences");
+    int max_rows = 0, rounds = 1;
+    for (const KvShiftSeq& q : seqs) {
+        max_rows = std::max(max_rows, std::min(q.n_rows, q.discard));
+        rounds = std::max(rounds, kv_shift_rounds(q.n_rows, q.discard));
+    }
+    CU(cudaMemcpyAsync(shift_seqs_, seqs.data(), seqs.size() * sizeof(KvShiftSeq), cudaMemcpyHostToDevice, stream_));      // pageable: staged before the call returns
+    const KvShiftParams p{kcache_, vcache_, kv_layer_elems_, shift_seqs_, (int)seqs.size(), n_layer_, n_kv_, hd_, rope_cos_, rope_sin_};
+    CU(kv_shift_launch(p, max_rows, rounds, stream_));
     return {};
 }
 
@@ -854,6 +881,24 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
     ST(plan_draw(so, true, &plan));
     for (int i = 0; i < n_prompt; ++i)
         if (prompt[i] < 0 || prompt[i] >= n_vocab_) return fail(GL_ERR_INVALID, "prompt token id out of range");
+    // context shift: an over-long prompt is cut to the positions a shift would leave; a sequence that outgrows the context
+    // shifts between decode chunks (the steps of a chunk never write past position W - 1)
+    const int W = n_ctx_;
+    int keep = 0, discard = 0;
+    bool shifting = false, cut = false;
+    std::vector<int32_t> cut_ids;
+    if (context_shift_) {
+        ST(shift_plan(so, n_prompt, n_pred, &keep));
+        discard = shift_discard(W, keep);
+        cut = n_prompt >= W;
+        shifting = cut || n_prompt + n_pred > W;
+        if (shifting && use_mega_) return fail(GL_ERR_UNSUPPORTED, "the persistent decode kernel (GL_MEGA=1) has no context shift");
+        if (cut) {
+            cut_ids.resize(W);
+            n_prompt = cut_prompt(prompt, n_prompt, W, keep, discard, cut_ids.data());
+            prompt = cut_ids.data();
+        }
+    }
     // prefix reuse: keep the pages of the positions the previous request left final and that this prompt repeats
     const int reuse = (prefix_cache_ && !use_mega_) ? prefix_reuse(prompt, n_prompt, cached_ids_.data(), (int)cached_ids_.size(), prefill_min_) : 0;
     if (reuse > 0) {
@@ -862,7 +907,7 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
     } else {
         ST(kv_reset());
     }
-    ST(ensure_pages(n_prompt + n_pred));
+    ST(ensure_pages(context_shift_ ? std::min(n_prompt + n_pred, W) : n_prompt + n_pred));
     if (so.want_logits) {
         if (keep_cap_ < n_pred) {
             float* p = nullptr;
@@ -903,8 +948,16 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
     bool cancelled = false;
     const int chunk = cb ? 8 : 32;
     StepState hs{};
+    int pos = batched ? n_prompt : n_prompt - 1;      // the position the chunk's first full step writes
+    int n_shifts = 0;
     while (produced < n_pred && !cancelled) {
-        const int n = std::min(chunk, n_pred - produced);
+        if (shifting && pos == W) {
+            // between chunks, in plain stream order: the kernel also lowers the device position by `discard`
+            ST(launch_shift({KvShiftSeq{page_table_, keep, discard, shift_rows(W, keep, discard), st_}}));
+            pos -= discard;
+            ++n_shifts;
+        }
+        const int n = shifting ? shift_chunk(chunk, n_pred - produced, pos, W, first_head_only) : std::min(chunk, n_pred - produced);
         int full = n;
         if (first_head_only) {
             int dummy = 0;
@@ -930,11 +983,12 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
             ++produced;
         }
         if (hs.done) { done_reason = 0; break; }
+        pos = hs.pos;
     }
     CU(cudaEventRecord(ev_[2], stream_));
     CU(cudaEventSynchronize(ev_[2]));
     if (cancelled) done_reason = 2;
-    host_pos_ = n_prompt + produced;
+    host_pos_ = n_shifts > 0 ? pos : n_prompt + produced;
     if (prefix_cache_ && !use_mega_) {
         // K / V are final for the prompt and for every generated id the device has FED: a step feeds output i - 1 while it draws
         // output i, so hs.out_idx draws fed hs.out_idx - 1 of them.  The last draw (and a stop token) was never fed; steps the
@@ -942,6 +996,8 @@ Status Engine::generate(const int32_t* prompt, int n_prompt, const gl_sample_opt
         const int fed = std::max(0, std::min(produced, hs.out_idx - 1));
         cached_ids_.assign(prompt, prompt + n_prompt);
         cached_ids_.insert(cached_ids_.end(), ids.begin(), ids.begin() + fed);
+        // after a cut or a shift only the kept positions [0, keep) hold the K / V of the ids recorded there
+        if (cut || n_shifts > 0) cached_ids_.resize(std::min<size_t>(cached_ids_.size(), (size_t)keep));
     }
     if (stats) {
         float ms_p = 0.f, ms_d = 0.f;

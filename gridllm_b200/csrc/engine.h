@@ -141,6 +141,14 @@ private:
     // single-sequence pages are final; cleared by everything else that writes those pages or the step state
     bool prefix_cache_ = false;
     std::vector<int32_t> cached_ids_;
+    // context shift (gl_engine_opts context_shift; rule in include/gridllm_native.h, context_shift.h)
+    bool context_shift_ = false;
+    KvShiftSeq* shift_seqs_ = nullptr;               // device [MAX_BATCH] sequence list of one kv_shift launch
+    // the keep count of a request whose prompt has n_prompt ids (GL_ERR_INVALID for num_keep < -1; num_keep is read only here,
+    // and only with the option on) and its num_predict bound
+    Status shift_plan(const gl_sample_opts& so, int n_prompt, int n_pred, int* keep);
+    // one kv_shift launch over these sequences (each moves shift_rows(W, keep, discard) rows)
+    Status launch_shift(const std::vector<KvShiftSeq>& seqs);
     const DevMatrix* find_matrix(const std::string& name) const;
 
     // model
@@ -236,6 +244,9 @@ private:
         int64_t prefill_ns = 0, eval_ns = 0, t_open_ns = 0;      // device time of its prefill / of the steps it took part in; host clock at open
         int launches = 0;
         bool stopped = false;                         // ended on a stop token
+        int pos = 0;                                  // position its next step writes (context shift)
+        int keep = 0;                                 // context shift: its keep count; shifts only when shift_on
+        bool shift_on = false;
     };
     static constexpr int N_BUCKETS = 5;               // batch-size buckets of the captured step: 8, 16, 32, 64, 128 rows
     int max_batch_ = 0;                               // gl_engine_opts.max_batch (0: batching off)
@@ -272,7 +283,8 @@ private:
     int batch_launches_ = 0;                          // kernels of one batched step (without the penalty / mask kernels)
     uint64_t bc_[8] = {};                             // gl_batch_counters
     Status ensure_batch_state();
-    Status seq_open_single(const int32_t* prompt, int n_prompt, const gl_sample_opts& so, int* slot);
+    // was_cut: the caller already cut this prompt (context shift), so it counts as a shifting sequence
+    Status seq_open_single(const int32_t* prompt, int n_prompt, const gl_sample_opts& so, int* slot, bool was_cut = false);
     Status enqueue_batch_step(cudaStream_t s, int bucket, bool penalised, bool masked, int* n_launch);
     Status run_batch_graph(int bucket, bool penalised, bool masked);
     int batch_checked_ = 0;                           // variant bits whose kernels have run once outside stream capture

@@ -18,6 +18,7 @@
 
 #include "common.cuh"
 #include "engine.h"
+#include "context_shift.h"
 
 namespace gl {
 
@@ -244,7 +245,9 @@ void Engine::index_prompt_pages(const int32_t* prompt, int n_prompt, const std::
 // packed pass does not take (shorter than 8 tokens, longer than a pack, no 16-bit weights) go through seq_open_single.
 Status Engine::seq_open(const int32_t* prompt, int n_prompt, const gl_sample_opts& so, int* slot_out) {
     if (!prompt || n_prompt <= 0 || !slot_out) return failb(GL_ERR_INVALID, "seq_open: empty prompt");
-    if (have_w16_ && prefill_mode_ != 1 && n_prompt >= prefill_min_ && n_prompt <= EMB_PACK_TOKENS) {
+    int n_eval = n_prompt;                            // what the prompt pass evaluates: a prompt of W ids or more is cut first
+    if (context_shift_ && n_prompt >= n_ctx_ && so.num_keep >= -1) n_eval = n_ctx_ - shift_discard(n_ctx_, shift_keep(so.num_keep, n_prompt, n_ctx_));
+    if (have_w16_ && prefill_mode_ != 1 && n_eval >= prefill_min_ && n_eval <= EMB_PACK_TOKENS) {
         const int32_t offs[2] = {0, n_prompt};
         int32_t slot = -1;
         int n = 0;
@@ -255,7 +258,7 @@ Status Engine::seq_open(const int32_t* prompt, int n_prompt, const gl_sample_opt
     return seq_open_single(prompt, n_prompt, so, slot_out);
 }
 
-Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sample_opts& so, int* slot_out) {
+Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sample_opts& so, int* slot_out, bool was_cut) {
     CU(cudaSetDevice(device_));
     if (!prompt || n_prompt <= 0 || !slot_out) return failb(GL_ERR_INVALID, "seq_open: empty prompt");
     for (int i = 0; i < n_prompt; ++i)
@@ -264,18 +267,33 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
     ST(plan_draw(so, false, &plan));
     ST(ensure_batch_state());
     const int n_pred = so.num_predict > 0 ? so.num_predict : 128;
-    if (n_prompt + n_pred > n_ctx_) return failb(GL_ERR_CONTEXT, "prompt + num_predict exceeds the engine context");
+    // context shift: cut an over-long prompt; a sequence that may shift reserves pages for W positions at most and shares none
+    int keep = 0, page_pred = n_pred;                 // pages for n_prompt + page_pred positions
+    bool shifting = false;
+    std::vector<int32_t> cut_ids;
+    if (context_shift_) {
+        ST(shift_plan(so, n_prompt, n_pred, &keep));
+        shifting = was_cut || n_prompt + n_pred > n_ctx_;
+        if (n_prompt >= n_ctx_) {
+            cut_ids.resize(n_ctx_);
+            n_prompt = cut_prompt(prompt, n_prompt, n_ctx_, keep, shift_discard(n_ctx_, keep), cut_ids.data());
+            prompt = cut_ids.data();
+        }
+        page_pred = std::min(n_pred, n_ctx_ - n_prompt);
+    } else if (n_prompt + n_pred > n_ctx_) {
+        return failb(GL_ERR_CONTEXT, "prompt + num_predict exceeds the engine context");
+    }
     int slot = -1;
     for (int i = 0; i < max_batch_; ++i)
         if (!slots_[i].open) { slot = i; break; }
     if (slot < 0) return failb(GL_ERR_NOMEM, "no free sequence slot (max_batch " + std::to_string(max_batch_) + ")");
     // pages for every position it will hold, reserved up front: a step can never run out.  Only a prompt that takes the prompt
     // pass shares a prefix (and indexes its pages afterwards); short prompts step through the decode kernels.
-    const bool share = share_prefixes() && can_batch_prefill(0, n_prompt);
+    const bool share = share_prefixes() && can_batch_prefill(0, n_prompt) && !shifting;
     SeqSlot& S = slots_[slot];
     S = SeqSlot{};
     int r = 0;
-    if (!take_pages(prompt, n_prompt, n_pred, share, &S.pages, &r)) return failb(GL_ERR_NOMEM, "KV page pool exhausted");
+    if (!take_pages(prompt, n_prompt, page_pred, share, &S.pages, &r)) return failb(GL_ERR_NOMEM, "KV page pool exhausted");
     int* table = btables_ + (size_t)slot * n_pages_;
     CU(cudaMemcpyAsync(table, S.pages.data(), S.pages.size() * 4, cudaMemcpyHostToDevice, stream_));
     if (plan.penalised) {                                 // the head of the history the batched steps penalise with
@@ -317,6 +335,7 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
         float pms = 0.f;
         cudaEventElapsedTime(&pms, ev_[2], ev_[3]);
         S.prefill_ns = (int64_t)(pms * 1e6);
+        S.pos = hs.pos;
         S.last_token = hs.token;
         S.first_lp = lp;
         S.done = hs.done != 0;
@@ -331,6 +350,7 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
     S.open = true;
     S.n_shared = r;
     S.n_prompt = n_prompt; S.n_pred = n_pred; S.produced = 0; S.plan = plan; S.first_pending = true;
+    S.keep = keep; S.shift_on = shifting;
     S.t_open_ns = t_open; S.launches = prefill_launches; S.stopped = S.done;
     bc_[3] += (uint64_t)S.prefill_ns; bc_[4] += (uint64_t)(n_prompt - r); bc_[5] += 1; bc_[6] += (uint64_t)prefill_launches;
     bc_[7] += (uint64_t)r;
@@ -349,6 +369,11 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
     *n_opened = 0;
     ST(ensure_batch_state());
     std::vector<DrawPlan> plans(n_seq);
+    // context shift: per prompt its keep count and whether it may shift (or was cut); over-long prompts are cut into a copy
+    std::vector<int> keeps(n_seq, 0);
+    std::vector<char> shifting(n_seq, 0);
+    std::vector<int32_t> cut_ids;
+    std::vector<int32_t> cut_offs;
     for (int i = 0; i < n_seq; ++i) {
         slots_out[i] = -1;
         const int n = offs[i + 1] - offs[i];
@@ -357,7 +382,25 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             if (ids[offs[i] + k] < 0 || ids[offs[i] + k] >= n_vocab_) return failb(GL_ERR_INVALID, "prompt token id out of range");
         ST(plan_draw(opts[i], false, &plans[i]));
         const int n_pred = opts[i].num_predict > 0 ? opts[i].num_predict : 128;
-        if (n + n_pred > n_ctx_) return failb(GL_ERR_CONTEXT, "prompt + num_predict exceeds the engine context");
+        if (context_shift_) {
+            ST(shift_plan(opts[i], n, n_pred, &keeps[i]));
+            shifting[i] = n + n_pred > n_ctx_;
+        } else if (n + n_pred > n_ctx_) {
+            return failb(GL_ERR_CONTEXT, "prompt + num_predict exceeds the engine context");
+        }
+    }
+    if (context_shift_) {
+        cut_offs.assign(1, 0);
+        for (int i = 0; i < n_seq; ++i) {
+            const int n = offs[i + 1] - offs[i];
+            const size_t at = cut_ids.size();
+            cut_ids.resize(at + n);
+            const int m = cut_prompt(ids + offs[i], n, n_ctx_, keeps[i], shift_discard(n_ctx_, keeps[i]), cut_ids.data() + at);
+            cut_ids.resize(at + m);
+            cut_offs.push_back((int32_t)cut_ids.size());
+        }
+        ids = cut_ids.data();
+        offs = cut_offs.data();
     }
     if (!pk_ids_) {
         auto dalloc = [&](void** p, size_t bytes) -> cudaError_t {
@@ -387,9 +430,11 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             const int n = offs[next + 1] - offs[next];
             if (!packable || n > EMB_PACK_TOKENS || n < prefill_min_) break;              // this one goes through gl_seq_open's own path
             // the positions a shared prefix covers are not evaluated: only the suffix takes rows of the pack
-            const int r_max = share ? shared_prefix_reuse(pages_.match(prompt, n, nullptr), n, prefill_min_) : 0;
+            const bool share_i = share && !shifting[next];
+            const int r_max = share_i ? shared_prefix_reuse(pages_.match(prompt, n, nullptr), n, prefill_min_) : 0;
             if (rows + (n - r_max + 127) / 128 * 128 > EMB_PACK_TOKENS) break;
-            const int n_pred = opts[next].num_predict > 0 ? opts[next].num_predict : 128;
+            int n_pred = opts[next].num_predict > 0 ? opts[next].num_predict : 128;
+            if (shifting[next]) n_pred = std::min(n_pred, n_ctx_ - n);         // pages for min(n_prompt + num_predict, W) positions
             int slot = -1;
             for (int k = 0; k < max_batch_; ++k)
                 if (!slots_[k].open && std::find(pslots.begin(), pslots.end(), k) == pslots.end()) { slot = k; break; }
@@ -397,12 +442,12 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             SeqSlot& S = slots_[slot];
             S = SeqSlot{};
             int r = 0;
-            if (!take_pages(prompt, n, n_pred, share, &S.pages, &r)) { out_of_room = true; break; }
+            if (!take_pages(prompt, n, n_pred, share_i, &S.pages, &r)) { out_of_room = true; break; }
             CU(cudaMemcpyAsync(btables_ + (size_t)slot * n_pages_, S.pages.data(), S.pages.size() * 4, cudaMemcpyHostToDevice, stream_));
             // its prompt pages go into the index now, so that later prompts of this pack share them: the QKV projection of every
             // layer writes this sequence's K / V rows to its pages before that layer's attention reads them through a sharer's
             // table (a sharer comes after its owner in the pack)
-            if (share) index_prompt_pages(prompt, n, S.pages, r / KV_PAGE_TOKENS, &indexed);
+            if (share_i) index_prompt_pages(prompt, n, S.pages, r / KV_PAGE_TOKENS, &indexed);
             const int len = n - r;
             std::memcpy(h_ids.data() + rows, prompt + r, (size_t)len * 4);
             starts.push_back(rows); lens.push_back(len); which.push_back(next); pslots.push_back(slot); shared.push_back(r);
@@ -414,7 +459,7 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             if (out_of_room) break;
             // a prompt the packed pass does not take (too short / too long / no 16-bit weights): the single-sequence open
             int slot = -1;
-            Status st = seq_open_single(ids + offs[next], offs[next + 1] - offs[next], opts[next], &slot);
+            Status st = seq_open_single(ids + offs[next], offs[next + 1] - offs[next], opts[next], &slot, shifting[next] != 0);
             if (!st.ok()) {
                 if (st.code == GL_ERR_NOMEM || *n_opened > 0) break;      // what was opened so far stays open and is reported
                 return st;
@@ -516,6 +561,9 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             S.produced = 0;
             S.first_pending = true;
             S.last_token = ho[i].token;
+            S.pos = ho[i].pos;
+            S.keep = keeps[w];
+            S.shift_on = shifting[w] != 0;
             S.first_lp = ho[i].logprob;
             S.done = ho[i].done != 0;
             S.stopped = S.done;
@@ -763,8 +811,19 @@ Status Engine::batch_step(int32_t* out_slots, int32_t* out_ids, float* out_lps, 
         masked = masked || slots_[rows[r]].plan.masked;
     }
     CU(cudaEventRecord(ev_[2], stream_));
+    // context shift: every row whose step would write position W first shifts its rows, all of them in one launch.  The
+    // captured step, BatchCtl and the page tables stay as they are: the position is read on the device.
+    std::vector<KvShiftSeq> shifts;
+    for (int r = 0; r < B; ++r) {
+        SeqSlot& S = slots_[rows[r]];
+        if (!S.shift_on || S.pos < n_ctx_) continue;
+        const int d = shift_discard(n_ctx_, S.keep);
+        shifts.push_back(KvShiftSeq{btables_ + (size_t)rows[r] * n_pages_, S.keep, d, shift_rows(n_ctx_, S.keep, d), bst_ + rows[r]});
+        S.pos -= d;
+    }
+    ST(launch_shift(shifts));
     ST(run_batch_graph(bucket, penalised, masked));
-    const int step_launches = batch_launches_ + (penalised ? 1 : 0) + (masked ? 1 : 0) + 1;
+    const int step_launches = batch_launches_ + (penalised ? 1 : 0) + (masked ? 1 : 0) + 1 + (shifts.empty() ? 0 : 1);
     for (int r = 0; r < B; ++r) {                    // sampled rows: the seeded top-k / top-p sampler of the single-sequence path
         const int slot = rows[r];
         if (slots_[slot].plan.sampler == 0) continue;
@@ -792,6 +851,7 @@ Status Engine::batch_step(int32_t* out_slots, int32_t* out_ids, float* out_lps, 
             continue;
         }
         S.last_token = ho[r].token;
+        S.pos = ho[r].pos;
         ++S.produced;
         if (S.produced >= S.n_pred) S.done = true;
         emit(rows[r], ho[r].token, ho[r].logprob, S.done ? 1 : 0);

@@ -99,7 +99,7 @@ struct EmbedParams {
     int cols;
     int row_bytes;
     StepState* st;
-    const int* prompt_ids;  // sequential prefill: token = prompt_ids[pos] while pos < n_prompt
+    const int* prompt_ids;  // sequential prefill: token = prompt_ids[pos] while pos < n_prompt and nothing was drawn yet
     float* x;
 };
 cudaError_t embed_launch(const EmbedParams& p, bool pdl, cudaStream_t s);
@@ -187,6 +187,34 @@ cudaError_t schema_mask_launch(const SchemaMaskParams& p, int rows, bool pdl, cu
 // one thread: e's automaton from the initial state through the pieces of ids[0..n-1), stored as entry (n - 1) & 1 (the mask
 // kernel of output n advances by ids[n-1] itself).  gl_constrain_logits.
 cudaError_t schema_replay_launch(SchemaSlot* e, const int* ids, int n, const uint32_t* offsets, const uint8_t* bytes, cudaStream_t s);
+
+// Context shift (kv_shift.cu; rule in include/gridllm_native.h): for each sequence of the list, the rows [keep + discard,
+// keep + discard + n_rows) of every layer and KV head move to [keep, keep + n_rows) of its paged cache, K rotated by -discard
+// positions (fp32 pair rotation with the cos / sin table row `discard`, rounded to fp16), V copied bit for bit; then
+// st->pos -= discard (st may be null).  HBM-bound: 16-byte loads and stores.
+// ORDERING: the batch-1 decode attention reads the position before its griddepcontrol.wait, on the promise that the position
+// only grows within a step; a shift makes it go down.  So the shift is launched WITHOUT programmatic dependent launch and never
+// executes griddepcontrol.launch_dependents: nothing of the next step starts before it completes.
+struct KvShiftSeq {
+    const int* table;       // the sequence's page table (logical -> physical page)
+    int keep, discard, n_rows;
+    StepState* st;
+};
+struct KvShiftParams {
+    __half* k_cache;        // layer 0 base, [layer][page][kv][16][head_dim]
+    __half* v_cache;
+    size_t layer_elems;     // elements of one layer of the pool
+    const KvShiftSeq* seqs; // device, [n_seq]
+    int n_seq;
+    int n_layer, n_kv, head_dim;
+    const float* cos_t;     // [n_ctx][head_dim / 2]
+    const float* sin_t;
+};
+// max_rows: the largest n_rows of the list.  A sequence whose discard is smaller than its n_rows (source and destination
+// overlap) moves its rows in launches of at most `discard` rows each, in increasing order: n_rounds = the largest
+// ceil(n_rows / discard) of the list (at least 1; one launch when no ranges overlap, the case of the rule's discard).
+int kv_shift_rounds(int n_rows, int discard);
+cudaError_t kv_shift_launch(const KvShiftParams& p, int max_rows, int n_rounds, cudaStream_t s);
 
 // standalone pieces (used for fp-weight models and as unfused cross-checks)
 cudaError_t rmsnorm_launch(const float* x, const float* w, int n, float eps, float* y, cudaStream_t s);

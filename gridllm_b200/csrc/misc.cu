@@ -56,7 +56,9 @@ __global__ void __launch_bounds__(256) embed_kernel(const __grid_constant__ Embe
         const int pos = __ldcg(&p.st->pos);
         const int np = __ldcg(&p.st->n_prompt);
         int tok = __ldcg(&p.st->token);
-        if (pos < np) tok = __ldcg(p.prompt_ids + pos);
+        // prompt positions step through here only before the first draw: after a context shift a generated token may sit at a
+        // position below n_prompt
+        if (pos < np && __ldcg(&p.st->out_idx) == 0) tok = __ldcg(p.prompt_ids + pos);
         if (blockIdx.x == 0) p.st->token = tok;       // same value every CTA derives: no ordering needed
         tok_s = tok;
     }

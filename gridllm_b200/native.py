@@ -57,6 +57,16 @@ class EngineOpts(C.Structure):
     def batch_prefix_cache(self, v: int) -> None:
         self.reserved[self.GL_OPT_BATCH_PREFIX_CACHE] = int(v)
 
+    GL_OPT_CONTEXT_SHIFT = 1               # include/gridllm_native.h: the reserved word that holds context_shift
+
+    @property
+    def context_shift(self) -> int:
+        return self.reserved[self.GL_OPT_CONTEXT_SHIFT]
+
+    @context_shift.setter
+    def context_shift(self, v: int) -> None:
+        self.reserved[self.GL_OPT_CONTEXT_SHIFT] = int(v)
+
 
 class ModelInfo(C.Structure):
     _fields_ = [("arch", C.c_char * 32), ("name", C.c_char * 96), ("quantization", C.c_char * 24),
@@ -81,7 +91,9 @@ class SampleOpts(C.Structure):
                 ("repeat_penalty", C.c_float), ("repeat_last_n", C.c_int32), ("presence_penalty", C.c_float),
                 ("frequency_penalty", C.c_float), ("min_p", C.c_float),
                 # output format (0 off, GL_FORMAT_JSON), in the union with the last reserved word
-                ("_fmt", _FormatWord)]
+                ("_fmt", _FormatWord),
+                # context shift: prompt positions a shift keeps (-1 the whole prompt); read only with Engine(context_shift=True)
+                ("num_keep", C.c_int32)]
 
 
 GL_FORMAT_JSON = 1
@@ -199,7 +211,7 @@ class Engine:
 
     def __init__(self, gguf_path: str, device: int = 0, max_ctx: int = 0, act_bits: int = 16, use_graph: bool = True,
                  use_pdl: bool = True, prefill_mode: int = 0, max_batch: int = 0, kv_pool_tokens: int = 0, batch_weights: int = 0,
-                 prefix_cache: bool = False, batch_prefix_cache: bool = False):
+                 prefix_cache: bool = False, batch_prefix_cache: bool = False, context_shift: bool = False):
         self._lib = load_library()
         self._h = C.c_void_p()
         o = EngineOpts()
@@ -211,6 +223,8 @@ class Engine:
         o.prefix_cache = int(bool(prefix_cache))
         # seq_open / seq_open_many sequences share the KV pages of prompt prefixes, also with closed ones (include/gridllm_native.h)
         o.batch_prefix_cache = int(bool(batch_prefix_cache))
+        # a sequence that fills the context keeps generating: over-long prompts are cut and the KV cache shifts (include/gridllm_native.h)
+        o.context_shift = int(bool(context_shift))
         _check(self._lib.gl_engine_create(gguf_path.encode(), device, C.byref(o), C.byref(self._h)))
         self.info = ModelInfo()
         _check(self._lib.gl_engine_info(self._h, C.byref(self.info)))
@@ -260,10 +274,11 @@ class Engine:
                  on_token: Optional[Callable[[int, float, bytes], bool]] = None, want_logits: bool = False,
                  stop_ids: Sequence[int] = (), temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0,
                  seed: int = 0, repeat_penalty: float = 1.0, repeat_last_n: int = 64, presence_penalty: float = 0.0,
-                 frequency_penalty: float = 0.0, min_p: float = 0.0, format: Optional[str] = None) -> Generation:
+                 frequency_penalty: float = 0.0, min_p: float = 0.0, format: Optional[str] = None, num_keep: int = 0) -> Generation:
         p = np.ascontiguousarray(prompt, dtype=np.int32)
         so = SampleOpts()
         so.num_predict, so.ignore_eos, so.want_logits = num_predict, int(ignore_eos), int(want_logits)
+        so.num_keep = int(num_keep)
         so.format = self._format(format)
         so.temperature, so.top_k, so.top_p, so.seed = float(temperature), int(top_k), float(top_p), int(seed) & (2**64 - 1)
         _set_penalties(so, dict(repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n, presence_penalty=presence_penalty,
@@ -292,10 +307,12 @@ class Engine:
     # ---- continuous batching (gl_seq_open / gl_batch_step / gl_seq_close) ---------------------------------
     def seq_open(self, prompt: Sequence[int], num_predict: int = 128, ignore_eos: bool = False, temperature: float = 0.0, top_k: int = 0,
                  top_p: float = 1.0, seed: int = 0, stop_ids: Sequence[int] = (), repeat_penalty: float = 1.0, repeat_last_n: int = 64,
-                 presence_penalty: float = 0.0, frequency_penalty: float = 0.0, min_p: float = 0.0, format: Optional[str] = None) -> int:
+                 presence_penalty: float = 0.0, frequency_penalty: float = 0.0, min_p: float = 0.0, format: Optional[str] = None,
+                 num_keep: int = 0) -> int:
         p = np.ascontiguousarray(prompt, dtype=np.int32)
         so = SampleOpts()
         so.num_predict, so.ignore_eos = (num_predict if num_predict > 0 else 128), int(ignore_eos)
+        so.num_keep = int(num_keep)
         so.format = self._format(format)
         so.temperature, so.top_k, so.top_p, so.seed = float(temperature), int(top_k), float(top_p), int(seed) & (2**64 - 1)
         _set_penalties(so, dict(repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n, presence_penalty=presence_penalty,
@@ -324,6 +341,7 @@ class Engine:
             so[i].seed = int(o.get("seed", 0)) & (2**64 - 1)
             _set_penalties(so[i], {k: o.get(k) for k in PENALTY_DEFAULTS})
             so[i].format = self._format(o.get("format"))
+            so[i].num_keep = int(o.get("num_keep", 0))
             stops = np.ascontiguousarray(o.get("stop_ids", ()), dtype=np.int32)
             keep.append(stops)
             so[i].n_stop_ids = len(stops)

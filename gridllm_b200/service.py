@@ -93,7 +93,7 @@ class NativeInferenceService:
     def __init__(self, models: Dict[str, str], device: int = 0, max_ctx: int = 0,
                  sampling_defaults: Optional[Dict[str, Any]] = None, apply_template: bool = False, max_batch: int = 0,
                  jinja_templates: bool = True, penalty_defaults: Optional[Dict[str, Any]] = None, json_schema: bool = False,
-                 **engine_kw):
+                 context_shift: bool = False, **engine_kw):
         """models: Ollama-style model name -> GGUF path.
         sampling_defaults: options a request inherits when it does not carry them.  None = greedy (temperature 0, the
         BASELINE.json configuration); pass OLLAMA_SAMPLING_DEFAULTS to behave like an Ollama worker for such requests.
@@ -107,6 +107,12 @@ class NativeInferenceService:
         json_schema: enforce a JSON-schema `format` (metadata.format or options.format) on the GPU: the response is a document
         of the schema, and a schema outside the supported subset fails the request before it runs.  False (default): a schema
         object only asks for valid JSON of any shape.
+        context_shift: keep answering when a conversation outgrows the engine's context, as Ollama does: a prompt of the
+        context's length or more is cut to its first options.num_keep tokens (default 4, -1 the whole prompt) plus its newest
+        ones, and a generation that reaches the context shifts the KV cache instead of stopping.  num_predict is then bounded
+        by the context itself (<= 0 means the context's length), not by what is left of it.  The returned context is still
+        the whole conversation as sent plus the reply.  Off by default: a generation ends at the context and a prompt that
+        does not fit fails.
         engine_kw: further Engine options, e.g. prefix_cache=True: a request keeps the KV pages of the longest prefix it shares
         with the previous request on the same engine (a multi-turn client that sends metadata.context back then pays for its
         new tokens only, as with Ollama's cached prefix), and its prompt_eval_count counts the tokens it evaluated.  Off by
@@ -117,6 +123,7 @@ class NativeInferenceService:
         self._sampling_defaults = dict(sampling_defaults or {})
         self._penalty_defaults = dict(penalty_defaults or {})
         self._json_schema = bool(json_schema)
+        self._context_shift = bool(context_shift)
         # Ollama wraps the prompt of /api/generate and /v1/completions in the model's template (system + prompt as one user
         # turn) unless the request says raw [external]; off by default: the prompt text is tokenised as it is
         self._apply_template = bool(apply_template)
@@ -125,10 +132,10 @@ class NativeInferenceService:
         self._paths = dict(models)
         self._device = device
         self._max_ctx = max_ctx
-        self._engine_kw = engine_kw
+        self._engine_kw = dict(engine_kw, context_shift=True) if self._context_shift else engine_kw
         self._max_batch = int(max_batch) if int(max_batch) > 1 else 0
         if self._max_batch:
-            self._engine_kw = dict(engine_kw, max_batch=self._max_batch)
+            self._engine_kw = dict(self._engine_kw, max_batch=self._max_batch)
         self._runners: Dict[str, Any] = {}
         self._engines: Dict[str, N.Engine] = {}
         self._lock = threading.Lock()          # one engine call at a time (one CUDA stream per engine)
@@ -166,6 +173,19 @@ class NativeInferenceService:
         if v is None or v == 0:
             return 128
         return int(v)
+
+    NUM_KEEP_DEFAULT = 4        # this project's choice (Ollama's own default is not pinned here)
+
+    @classmethod
+    def _num_keep(cls, options: Dict[str, Any]) -> int:
+        """options.num_keep: the prompt tokens a context shift keeps; absent -> 4, -1 the whole prompt"""
+        v = options.get("num_keep")
+        if v is None:
+            return cls.NUM_KEEP_DEFAULT
+        v = int(v)
+        if v < -1:
+            raise RuntimeError("num_keep must be >= -1")
+        return v
 
     def close(self):
         for r in self._runners.values():
@@ -355,10 +375,18 @@ class NativeInferenceService:
         # a generation that would run past the engine's context ends at it (done_reason "length") instead of failing; a prompt
         # that does not fit at all still fails (GL_ERR_CONTEXT)
         n_ctx = int(getattr(eng.info, "n_ctx", 0) or 0)
-        if num_predict <= 0:                             # -1 / -2: until EOS, bounded by the context
-            num_predict = max(1, n_ctx - len(ids)) if n_ctx > 0 else 128
-        if n_ctx > 0 and len(ids) < n_ctx:
-            num_predict = min(num_predict, n_ctx - len(ids))
+        if getattr(self, "_context_shift", False):
+            # the cache shifts instead: only the output buffers (n_ctx ids) bound a generation
+            if n_ctx > 0:
+                num_predict = n_ctx if num_predict <= 0 else min(num_predict, n_ctx)
+            elif num_predict <= 0:
+                num_predict = 128
+            kw["num_keep"] = self._num_keep(options)
+        else:
+            if num_predict <= 0:                             # -1 / -2: until EOS, bounded by the context
+                num_predict = max(1, n_ctx - len(ids)) if n_ctx > 0 else 128
+            if n_ctx > 0 and len(ids) < n_ctx:
+                num_predict = min(num_predict, n_ctx - len(ids))
         stops = options.get("stop")
         stops = [stops] if isinstance(stops, str) else list(stops or [])
         if not stops or not eng.info.has_tokenizer:

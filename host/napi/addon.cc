@@ -84,6 +84,12 @@ napi_value CreateEngine(napi_env env, napi_callback_info info) {
             if (napi_get_value_bool(env, v, &b) == napi_ok) w = b ? 1 : 0;
             else napi_get_value_int32(env, v, &w);
         }
+        if (napi_get_named_property(env, argv[2], "contextShift", &v) == napi_ok) {      // boolean (or 0 / 1)
+            bool b = false;
+            int32_t& w = o.reserved[GL_OPT_CONTEXT_SHIFT];
+            if (napi_get_value_bool(env, v, &b) == napi_ok) w = b ? 1 : 0;
+            else napi_get_value_int32(env, v, &w);
+        }
     }
     o.use_graph = 1;
     o.use_pdl = 1;
@@ -104,6 +110,8 @@ void read_penalty_opts(napi_env env, napi_value o, gl_sample_opts& so) {
     if (napi_get_named_property(env, o, "presencePenalty", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.presence_penalty = (float)d;
     if (napi_get_named_property(env, o, "frequencyPenalty", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.frequency_penalty = (float)d;
     if (napi_get_named_property(env, o, "minP", &v) == napi_ok && napi_get_value_double(env, v, &d) == napi_ok) so.min_p = (float)d;
+    // context shift: the prompt positions a shift keeps (-1 the whole prompt); the engine reads it only with contextShift on
+    if (napi_get_named_property(env, o, "numKeep", &v) == napi_ok) napi_get_value_int32(env, v, &so.num_keep);
     // output format: "json" (or GL_FORMAT_JSON) turns the JSON grammar mask on, a formatSchema code the schema mask; absent, ""
     // or 0 is free text; anything else reaches the library as it is and is refused there (GL_ERR_INVALID)
     napi_valuetype vt;

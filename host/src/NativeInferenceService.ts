@@ -30,13 +30,16 @@ export class NativeInferenceService {
 	// (a client that sends `context` back pays for its new tokens only); off by default (include/gridllm_native.h).
 	// batchPrefixCache: the same for an engine created with maxBatch > 1: its sequences share the KV pages of prompt prefixes,
 	// with each other and with closed ones; off by default.
-	private engineOptions: { prefixCache?: boolean; batchPrefixCache?: boolean };
+	// contextShift: a conversation that outgrows the engine's context keeps being answered (over-long prompts cut to numKeep
+	// plus the newest tokens, the KV cache shifted while generating); off by default.  Same switch as service.py's context_shift.
+	private engineOptions: { prefixCache?: boolean; batchPrefixCache?: boolean; contextShift?: boolean };
 	// jsonSchema: enforce a JSON-schema `format` on the GPU (gl_format_schema); off by default: a schema asks for valid JSON of
 	// any shape, as before.  Same switch as gridllm_b200/service.py's json_schema.
 	private jsonSchema: boolean;
 
-	constructor(options: { prefixCache?: boolean; batchPrefixCache?: boolean; jsonSchema?: boolean } = {}) {
-		this.engineOptions = { prefixCache: !!options.prefixCache, batchPrefixCache: !!options.batchPrefixCache };
+	constructor(options: { prefixCache?: boolean; batchPrefixCache?: boolean; jsonSchema?: boolean; contextShift?: boolean } = {}) {
+		this.engineOptions = { prefixCache: !!options.prefixCache, batchPrefixCache: !!options.batchPrefixCache,
+			contextShift: !!options.contextShift };
 		this.jsonSchema = !!options.jsonSchema;
 	}
 
@@ -161,9 +164,17 @@ export class NativeInferenceService {
 		if (!(temperature >= 0) || !Number.isFinite(temperature)) throw new Error("temperature must be a finite number >= 0");
 		let numPredict = o.num_predict || 128;
 		const nCtx = e ? (native.engineInfo(e).nCtx as number) : 0;
-		if (numPredict < 0) numPredict = nCtx > 0 ? Math.max(1, nCtx - nPrompt) : 128;
-		if (nCtx > 0 && nPrompt < nCtx) numPredict = Math.min(numPredict, nCtx - nPrompt);
-		return { numPredict, ignoreEos: !!o.ignore_eos, temperature, topK: o.top_k ?? d.top_k ?? 0, topP: o.top_p ?? d.top_p ?? 1,
+		let numKeep: number | undefined;
+		if (this.engineOptions.contextShift) {
+			// the cache shifts: only the output buffers (nCtx ids) bound a generation; num_keep absent -> 4, -1 the whole prompt
+			if (nCtx > 0) numPredict = numPredict < 0 ? nCtx : Math.min(numPredict, nCtx);
+			numKeep = o.num_keep ?? 4;
+			if (numKeep < -1) throw new Error("num_keep must be >= -1");
+		} else {
+			if (numPredict < 0) numPredict = nCtx > 0 ? Math.max(1, nCtx - nPrompt) : 128;
+			if (nCtx > 0 && nPrompt < nCtx) numPredict = Math.min(numPredict, nCtx - nPrompt);
+		}
+		return { numPredict, ...(numKeep === undefined ? {} : { numKeep }), ignoreEos: !!o.ignore_eos, temperature, topK: o.top_k ?? d.top_k ?? 0, topP: o.top_p ?? d.top_p ?? 1,
 			seed: BigInt(o.seed ?? (temperature > 0 ? Math.floor(Math.random() * 2 ** 53) : 0)), ...this.penaltyOpts(o),
 			...this.formatOpts(request, e) };
 	}

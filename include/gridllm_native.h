@@ -87,11 +87,32 @@ typedef struct gl_engine_opts {
      * free pages first, then evicts retained pages, least recently released leaves first: GL_ERR_NOMEM comes only when open
      * sequences hold the pool.  gl_gen_stats.prompt_eval_count of gl_seq_stats counts the evaluated tokens and
      * prompt_eval_duration their share of the pass; gl_batch_counters out[7] counts the prompt tokens taken from shared pages.
-     * No sharing under GL_PREFILL_FLASH=0 or the persistent decode kernel (GL_MEGA=1).  The other reserved words must be 0. */
+     * No sharing under GL_PREFILL_FLASH=0 or the persistent decode kernel (GL_MEGA=1).
+     * reserved[GL_OPT_CONTEXT_SHIFT] is context_shift (Ollama's context shift): 0 = off, nothing below applies and a sequence
+     * longer than the context is GL_ERR_CONTEXT.  With it on, gl_generate, gl_seq_open and gl_seq_open_many keep generating
+     * when a sequence fills the context W = gl_model_info.n_ctx, and cut prompts of W tokens or more.  Let k be the request's
+     * keep count (gl_sample_opts.num_keep, read only when this option is on: >= 0 clamped to min(num_keep, W - 1), -1 the whole
+     * prompt clamped to W - 1, < -1 GL_ERR_INVALID) and d = ceil((W - k) / 2) >= 1 the discard:
+     *   - shift: when the next step of a sequence must write the row at position W, positions [k, k + d) are dropped and the
+     *     rows [k + d, W) move to [k, W - d), each K row rotated by -d positions (the pair rotation with the engine's fp32
+     *     cos / sin table row d, rounded to fp16), V rows copied bit for bit; rows [0, k) are untouched and the step runs at
+     *     position W - d.  Moved rows keep the context they were computed in.  The penalty history (prompt, then every
+     *     generated id), the grammar-mask state, the output index and the seeded draw (seed, i) are unchanged by a shift.
+     *   - prompt cut: a prompt of n_prompt >= W ids is cut to its first k ids plus its newest W - d - k ids (the positions a
+     *     shift would leave) and evaluated by one cold prompt pass; prompt_eval_count counts the evaluated ids and the penalty
+     *     history starts with the cut prompt.
+     *   - num_predict <= W (the output buffers hold W ids); more is GL_ERR_CONTEXT.  Pages are reserved for
+     *     min(n_prompt + num_predict, W) positions.
+     *   - a sequence with n_prompt + num_predict > W (one that may shift or was cut) neither reads nor indexes shared prompt
+     *     pages (batch_prefix_cache), and after gl_generate of such a sequence the prefix_cache record keeps positions [0, k)
+     *     only.  Sequences that fit behave exactly as with the option off.
+     *   - under the persistent decode kernel (GL_MEGA=1) a gl_generate that would cut or shift is GL_ERR_UNSUPPORTED.
+     * The other reserved words must be 0. */
     int32_t reserved[7];
 } gl_engine_opts;
 
 #define GL_OPT_BATCH_PREFIX_CACHE 0       /* index of batch_prefix_cache in gl_engine_opts.reserved */
+#define GL_OPT_CONTEXT_SHIFT 1            /* index of context_shift in gl_engine_opts.reserved */
 
 typedef struct gl_model_info {
     char     arch[32];
@@ -161,6 +182,10 @@ typedef struct gl_sample_opts {
         int32_t  format;
         int32_t  reserved[1];
     };
+    /* Ollama's num_keep: the prompt positions a context shift keeps (see gl_engine_opts context_shift): >= 0 that many, -1 the
+     * whole prompt.  Read only when the engine's context_shift option is on (a caller built against an older header may leave
+     * this word, then tail padding, uninitialised). */
+    int32_t  num_keep;
 } gl_sample_opts;
 
 #define GL_FORMAT_JSON 1
@@ -203,7 +228,9 @@ int  gl_chat_template(const gl_engine* e, char* buf, int32_t cap, int32_t* len_o
  * gl_generate: generateResponse / generateStreamResponse / generateChat*Response
  *   (OllamaService.ts:97-184, 186-284, 353-449, 451-599): prefill the prompt, then decode up to
  *   num_predict tokens; cb (may be NULL) is invoked once per generated token in order.
- *   out_ids / out_logprobs (may be NULL) receive up to num_predict entries. */
+ *   out_ids / out_logprobs (may be NULL) receive up to num_predict entries.  With gl_engine_opts context_shift on, a prompt of
+ *   the context's length or more is cut and generation goes on past the context by shifting the KV cache (rule, bounds and
+ *   interactions: gl_engine_opts context_shift). */
 int  gl_generate(gl_engine* e, const int32_t* prompt, int32_t n_prompt, const gl_sample_opts* opts,
                  gl_token_cb cb, void* user, int32_t* out_ids, float* out_logprobs, gl_gen_stats* stats);
 /* gl_embed: generateEmbedding (OllamaService.ts:601-665): prefill only, output_norm, mean-pool,
@@ -218,6 +245,9 @@ int  gl_embed(gl_engine* e, const int32_t* ids, const int32_t* seq_offsets, int3
  *                 gl_batch_step); pages for n_prompt + num_predict tokens are reserved up front, so a step cannot run out
  *                 (with batch_prefix_cache, less the prompt prefix it shares).
  *                 GL_ERR_NOMEM when no slot / not enough pages are free -- the caller may retry after a gl_seq_close.
+ *                 With context_shift on (gl_engine_opts), a prompt of the context's length or more is cut, pages for
+ *                 min(n_prompt + num_predict, W) positions are reserved, and gl_batch_step shifts the KV rows of every
+ *                 sequence that reaches the context in one launch before the step.
  *   gl_batch_step one token for every open, unfinished sequence.  Entry i: slots[i], ids[i], logprobs[i], done[i].
  *                 done = 1 with id >= 0: that token was the sequence's last (num_predict reached);  done = 1 with id = -1:
  *                 the token drawn was a stop token (not part of the output).  Finished sequences stay open, holding
