@@ -374,7 +374,7 @@ Status Engine::load(const std::string& path, int device, const gl_engine_opts* o
     info_.decode_bytes_per_token = decode_bytes_; info_.device = device_; info_.sm_count = sm_count_;
 
     ST(kv_reset());
-    if (prefill_mode_ != 1) ST(build_prefill_weights());
+    ST(build_prefill_weights(env_int("GL_PREFILL_WEIGHTS", 0)));
     // the persistent single-launch decode kernel is opt-in: it is correct (same tests) but, as of round 1, slower than
     // the per-op graph path
     if (fused_ && all_quant_ && env_int("GL_MEGA", 0) != 0) ST(build_mega());
@@ -1376,7 +1376,7 @@ Status Engine::embed(const int32_t* ids, const int32_t* offs, int n_seq, float* 
         CU(dalloc((void**)&emb_out_, (size_t)n_seq * n_embd_ * 4));
         emb_out_cap_ = n_seq;
     }
-    const bool packed = have_w16_ && prefill_mode_ != 1;
+    const bool packed = prefill_w_ != PREFILL_W_NONE;
     float* d_rows = nullptr;                               // sequential path only
     CU(cudaEventRecord(ev_[0], stream_));
     if (packed) {
@@ -1433,7 +1433,7 @@ Status Engine::embed(const int32_t* ids, const int32_t* offs, int n_seq, float* 
             }
         }
     } else {
-        // no 16-bit copy (prefill_mode 1 / not enough HBM): every sequence steps through the decode kernels, hidden state kept per position
+        // no prompt pass (prefill_mode 1): every sequence steps through the decode kernels, hidden state kept per position
         CU(cudaMalloc((void**)&d_rows, (size_t)max_n * n_embd_ * 4));
         Status st;
         for (int sidx = 0; sidx < n_seq && st.ok(); ++sidx) {

@@ -14,6 +14,7 @@
 #include "gguf_file.h"
 #include "kernels.h"
 #include "prefill.h"
+#include "prefill_weights.h"
 #include "batch.h"
 #include "qgemm.h"
 #include "decode_mega.h"
@@ -36,7 +37,7 @@ struct LayerWeights {
     float* attn_norm = nullptr;
     float* ffn_norm = nullptr;
     DevMatrix wq, wk, wv, wo, wgate, wup, wdown;
-    // resident 16-bit copies for the batched tensor-core prefill (built on the GPU at load)
+    // resident 16-bit copies for the batched tensor-core prefill (built on the GPU at load; null when the pass streams them)
     void* wqkv16 = nullptr;   // [(qd + 2 kvd) x n_embd]
     void* wo16 = nullptr;     // [n_embd x qd]
     void* wgu16 = nullptr;    // [2 n_ff x n_embd], rows interleaved 8 gate / 8 up
@@ -115,7 +116,12 @@ private:
     cudaError_t enqueue_pre_draw(cudaStream_t s, int bucket, bool penalised, bool masked, const int* prompt = nullptr, int* n_launch = nullptr);
     Status run_steps(int n_nohead, int n_head, bool keep_logits);
     Status enqueue_head(cudaStream_t s, bool keep_logits, int* n_launch);
-    Status build_prefill_weights();
+    Status build_prefill_weights(int request);       // request: GL_PREFILL_WEIGHTS (prefill_weights.h)
+    // the four 16-bit GEMM operands of a layer, in the layout of the resident copy
+    enum PrefillOperand { OP_QKV = 0, OP_O = 1, OP_GU = 2, OP_DOWN = 3 };
+    Status dequant_operand(const LayerWeights& L, PrefillOperand op, void* dst);
+    // operand op of layer L for a prompt-pass GEMM: the resident copy, or the staging buffer after one dequant launch (counted in *nl)
+    Status prompt_operand(const LayerWeights& L, PrefillOperand op, const void** b, int* nl);
     Status build_mega();
     Status launch_mega(int n_steps, bool with_head, bool keep_logits);
     Status ensure_prefill_scratch(int t_pad);
@@ -135,7 +141,7 @@ private:
     // n tokens from position pos0 through the tensor-core prompt pass; a pass that does not start at 0 (a later chunk of a long
     // prompt included) needs the fused prompt attention, so under GL_PREFILL_FLASH=0 such a prompt stays sequential
     bool can_batch_prefill(int pos0, int n) const {
-        return have_w16_ && prefill_mode_ != 1 && n >= prefill_min_ && (prefill_flash_ || (pos0 == 0 && n <= PF_CHUNK));
+        return prefill_w_ != PREFILL_W_NONE && n >= prefill_min_ && (prefill_flash_ || (pos0 == 0 && n <= PF_CHUNK));
     }
     // gl_generate's prefix reuse (gl_engine_opts.prefix_cache): ids at positions [0, cached_ids_.size()) whose K / V in the
     // single-sequence pages are final; cleared by everything else that writes those pages or the step state
@@ -179,7 +185,9 @@ private:
     bool use_graph_ = true, use_pdl_ = true, fused_ = true;
     int smem_kb_ = 224, attn_splits_ = 16;
     int prefill_mode_ = 0, prefill_min_ = 8;
-    bool have_w16_ = false, prefill_bf16_ = false, prefill_tc5_ = true;
+    int prefill_w_ = PREFILL_W_NONE;  // where the prompt pass reads its 16-bit weights (prefill_weights.h; GL_PREFILL_WEIGHTS)
+    void* w16_stage_ = nullptr;       // streamed: the one operand the next GEMM reads, [largest operand] 16-bit
+    bool prefill_bf16_ = false, prefill_tc5_ = true;
     bool prefill_fuse_rope_ = true;  // RoPE / split / cache append in the QKV GEMM's epilogue (GL_PREFILL_FUSE_ROPE=0: the stand-alone kernel)
     bool prefill_flash_ = true;     // fused prompt attention (prefill_attn.cu); GL_PREFILL_FLASH=0: the three-launch path, for A/B runs
     // prefill scratch (grown on demand)

@@ -134,7 +134,7 @@ Status Engine::ensure_batch_state() {
     if (batch_ready_) return {};
     if (bst_) return failb(GL_ERR_CUDA, "continuous batching: an earlier initialisation failed on this engine");
     if (max_batch_ < 2) return failb(GL_ERR_UNSUPPORTED, "continuous batching is off: create the engine with gl_engine_opts.max_batch >= 2");
-    if (!have_w16_) return failb(GL_ERR_UNSUPPORTED, "continuous batching needs the resident 16-bit weights (not enough HBM at load, or prefill_mode 1)");
+    if (prefill_w_ != PREFILL_W_RESIDENT) return failb(GL_ERR_UNSUPPORTED, "continuous batching needs the resident 16-bit weights (not enough HBM at load, or prefill_mode 1)");
     if (n_ff_ % 8) return failb(GL_ERR_UNSUPPORTED, "continuous batching: n_ff must be a multiple of 8");
     const int qd = n_head_ * hd_, kvd = n_kv_ * hd_, ldq = qd + 2 * kvd;
     auto dalloc = [&](void** p, size_t bytes) -> cudaError_t {
@@ -165,8 +165,12 @@ Status Engine::ensure_batch_state() {
     CU(dalloc((void**)&bsample_scratch_, R * BATCH_SAMPLE_ROW_FLOATS * 4));
     // the lm_head as a 16-bit matrix (the layer matrices already have their copy: build_prefill_weights)
     CU(dalloc(&head16_, (size_t)n_vocab_ * n_embd_ * 2));
-    CU(dequant_rows_launch(output_.w, output_.type, output_.rows, output_.cols, output_.row_stride, output_.tile_rows, head16_, n_embd_, 0, 0, false,
-                           stream_));
+    {
+        DequantOp op{};
+        op.src[0] = {output_.w, output_.type, output_.rows, output_.row_stride, output_.tile_rows, 0, 0};
+        op.n_src = 1; op.cols = n_embd_; op.dst = head16_;
+        CU(dequant_launch(op, false, stream_));
+    }
     CU(dalloc((void**)&bst_, sizeof(StepState) * R));
     CU(cudaStreamSynchronize(stream_));
     if (batch_weights_ != 1) {
@@ -247,7 +251,7 @@ Status Engine::seq_open(const int32_t* prompt, int n_prompt, const gl_sample_opt
     if (!prompt || n_prompt <= 0 || !slot_out) return failb(GL_ERR_INVALID, "seq_open: empty prompt");
     int n_eval = n_prompt;                            // what the prompt pass evaluates: a prompt of W ids or more is cut first
     if (context_shift_ && n_prompt >= n_ctx_ && so.num_keep >= -1) n_eval = n_ctx_ - shift_discard(n_ctx_, shift_keep(so.num_keep, n_prompt, n_ctx_));
-    if (have_w16_ && prefill_mode_ != 1 && n_eval >= prefill_min_ && n_eval <= EMB_PACK_TOKENS) {
+    if (prefill_w_ == PREFILL_W_RESIDENT && n_eval >= prefill_min_ && n_eval <= EMB_PACK_TOKENS) {
         const int32_t offs[2] = {0, n_prompt};
         int32_t slot = -1;
         int n = 0;
@@ -412,7 +416,7 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
         CU(dalloc((void**)&emb_pooled_, (size_t)n_embd_ * 4));
         CU(dalloc((void**)&emb_rstd_, (size_t)std::max(EMB_PACK_TOKENS, n_ctx_) * 4));
     }
-    const bool packable = have_w16_ && prefill_mode_ != 1;
+    const bool packable = prefill_w_ == PREFILL_W_RESIDENT;
     const bool share = packable && share_prefixes();
     const int64_t t_open = std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now().time_since_epoch()).count();
     int next = 0;

@@ -21,41 +21,73 @@ Status failp(int code, const std::string& m) { return Status{code, m}; }
     } while (0)
 }  // namespace
 
-// Resident 16-bit copy of every layer matrix, dequantised on the GPU from the engine layouts.
-// 2 bytes/weight (16 GB for Llama-3-8B) of the 80 GB HBM buys a prefill that never touches the
-// 4-bit decode layout.  fp16 is used for every model type (what ggml's CUDA backend also does for
+// The prompt pass's 16-bit layer matrices (prefill_weights.h).  Resident: a copy of every layer matrix, dequantised on the GPU
+// from the engine layouts -- 2 bytes/weight (14 GB for Llama-3-8B) of the 80 GB HBM buys a prefill that never touches the 4-bit
+// decode layout.  Streamed (the copy does not fit, e.g. 137 GB for a 70B): one staging buffer the size of the largest operand,
+// filled before each GEMM by prompt_operand.  fp16 is used for every model type (what ggml's CUDA backend also does for
 // batched matmuls [external]); bf16 weights convert to fp16 exactly within fp16's normal range.
-Status Engine::build_prefill_weights() {
+Status Engine::build_prefill_weights(int request) {
     const int qd = n_head_ * hd_, kvd = n_kv_ * hd_;
-    const size_t per_layer = ((size_t)(qd + 2 * kvd) * n_embd_ + (size_t)n_embd_ * qd + (size_t)2 * n_ff_ * n_embd_ + (size_t)n_embd_ * n_ff_) * 2;
     size_t free_b = 0, total_b = 0;
     CU(cudaMemGetInfo(&free_b, &total_b));
-    if (per_layer * n_layer_ + ((size_t)4 << 30) > free_b) {
-        have_w16_ = false;          // not enough HBM: prompts fall back to the sequential path (still on the GPU)
-        return {};
-    }
+    const uint64_t copy = prefill_copy_bytes(n_layer_, n_embd_, n_head_, n_kv_, hd_, n_ff_);
+    const int src = prefill_weights_source(prefill_mode_, request, copy, free_b);
+    if (src < 0)
+        return failp(GL_ERR_NOMEM, "GL_PREFILL_WEIGHTS=1: the resident 16-bit copy of the layer matrices needs " + std::to_string(copy >> 20) +
+                                       " MiB + 4096 MiB spare, " + std::to_string(free_b >> 20) + " MiB of HBM are free");
+    prefill_w_ = src;
+    if (src == PREFILL_W_NONE) return {};
+    if (n_ff_ % 8) return failp(GL_ERR_UNSUPPORTED, "n_ff must be a multiple of 8 for the batched prefill");
     auto alloc = [&](void** p, size_t elems) -> cudaError_t {
         cudaError_t e = cudaMalloc(p, elems * 2);
         if (e == cudaSuccess) allocs_.push_back(*p);
         return e;
     };
+    if (src == PREFILL_W_STREAMED) {
+        CU(alloc(&w16_stage_, prefill_stage_bytes(n_embd_, n_head_, n_kv_, hd_, n_ff_) / 2));
+        return {};
+    }
     for (int il = 0; il < n_layer_; ++il) {
         LayerWeights& L = layers_[il];
         CU(alloc(&L.wqkv16, (size_t)(qd + 2 * kvd) * n_embd_));
         CU(alloc(&L.wo16, (size_t)n_embd_ * qd));
         CU(alloc(&L.wgu16, (size_t)2 * n_ff_ * n_embd_));
         CU(alloc(&L.wd16, (size_t)n_embd_ * n_ff_));
-        if (n_ff_ % 8) return failp(GL_ERR_UNSUPPORTED, "n_ff must be a multiple of 8 for the batched prefill");
-        CU(dequant_rows_launch(L.wq.w, L.wq.type, L.wq.rows, L.wq.cols, L.wq.row_stride, L.wq.tile_rows, L.wqkv16, n_embd_, 0, 0, prefill_bf16_, stream_));
-        CU(dequant_rows_launch(L.wk.w, L.wk.type, L.wk.rows, L.wk.cols, L.wk.row_stride, L.wk.tile_rows, L.wqkv16, n_embd_, qd, 0, prefill_bf16_, stream_));
-        CU(dequant_rows_launch(L.wv.w, L.wv.type, L.wv.rows, L.wv.cols, L.wv.row_stride, L.wv.tile_rows, L.wqkv16, n_embd_, qd + kvd, 0, prefill_bf16_, stream_));
-        CU(dequant_rows_launch(L.wo.w, L.wo.type, L.wo.rows, L.wo.cols, L.wo.row_stride, L.wo.tile_rows, L.wo16, qd, 0, 0, prefill_bf16_, stream_));
-        CU(dequant_rows_launch(L.wgate.w, L.wgate.type, L.wgate.rows, L.wgate.cols, L.wgate.row_stride, L.wgate.tile_rows, L.wgu16, n_embd_, 0, 1, prefill_bf16_, stream_));
-        CU(dequant_rows_launch(L.wup.w, L.wup.type, L.wup.rows, L.wup.cols, L.wup.row_stride, L.wup.tile_rows, L.wgu16, n_embd_, 0, 2, prefill_bf16_, stream_));
-        CU(dequant_rows_launch(L.wdown.w, L.wdown.type, L.wdown.rows, L.wdown.cols, L.wdown.row_stride, L.wdown.tile_rows, L.wd16, n_ff_, 0, 0, prefill_bf16_, stream_));
+        ST(dequant_operand(L, OP_QKV, L.wqkv16));
+        ST(dequant_operand(L, OP_O, L.wo16));
+        ST(dequant_operand(L, OP_GU, L.wgu16));
+        ST(dequant_operand(L, OP_DOWN, L.wd16));
     }
     CU(cudaStreamSynchronize(stream_));
-    have_w16_ = true;
+    return {};
+}
+
+Status Engine::dequant_operand(const LayerWeights& L, PrefillOperand op, void* dst) {
+    auto src = [](const DevMatrix& m, int row0, int interleave) {
+        return DequantSrc{m.w, m.type, m.rows, m.row_stride, m.tile_rows, row0, interleave};
+    };
+    const int qd = n_head_ * hd_, kvd = n_kv_ * hd_;
+    DequantOp d{};
+    d.dst = dst;
+    switch (op) {
+        case OP_QKV: d.src[0] = src(L.wq, 0, 0); d.src[1] = src(L.wk, qd, 0); d.src[2] = src(L.wv, qd + kvd, 0); d.n_src = 3; d.cols = n_embd_; break;
+        case OP_O: d.src[0] = src(L.wo, 0, 0); d.n_src = 1; d.cols = qd; break;
+        case OP_GU: d.src[0] = src(L.wgate, 0, 1); d.src[1] = src(L.wup, 0, 2); d.n_src = 2; d.cols = n_embd_; break;
+        case OP_DOWN: d.src[0] = src(L.wdown, 0, 0); d.n_src = 1; d.cols = n_ff_; break;
+    }
+    CU(dequant_launch(d, prefill_bf16_, stream_));
+    return {};
+}
+
+Status Engine::prompt_operand(const LayerWeights& L, PrefillOperand op, const void** b, int* nl) {
+    if (prefill_w_ == PREFILL_W_RESIDENT) {
+        *b = op == OP_QKV ? L.wqkv16 : op == OP_O ? L.wo16 : op == OP_GU ? L.wgu16 : L.wd16;
+        return {};
+    }
+    // stream order alone makes the reuse safe: the GEMM that read the previous operand precedes this launch on stream_
+    ST(dequant_operand(L, op, w16_stage_));
+    ++*nl;
+    *b = w16_stage_;
     return {};
 }
 
@@ -133,7 +165,8 @@ Status Engine::prefill_chunk(int pos0, int n, int* n_launch) {
         bool roped = false;
         {
             GemmParams g{};
-            g.a = pf_xn_; g.b = L.wqkv16; g.c = pf_qkv_; g.m = T; g.n = ldq; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = ldq;
+            ST(prompt_operand(L, OP_QKV, &g.b, &nl));
+            g.a = pf_xn_; g.c = pf_qkv_; g.m = T; g.n = ldq; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = ldq;
             g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_F32;
             RopeSplitArgs ra{rope_cos_, rope_sin_, pf_q_, pf_k_, pf_vt_, kc, vc, n_head_, n_kv_, hd_, tp, segs};
             if (prefill_flash_ && prefill_fuse_rope_ && prefill_tc5_) {
@@ -170,20 +203,23 @@ Status Engine::prefill_chunk(int pos0, int n, int* n_launch) {
         }
         {
             GemmParams g{};
-            g.a = pf_attn_; g.b = L.wo16; g.c = pf_x_; g.m = T; g.n = n_embd_; g.k = qd; g.lda = qd; g.ldb = qd; g.ldc = n_embd_;
+            ST(prompt_operand(L, OP_O, &g.b, &nl));
+            g.a = pf_attn_; g.c = pf_x_; g.m = T; g.n = n_embd_; g.k = qd; g.lda = qd; g.ldb = qd; g.ldc = n_embd_;
             g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_ADD_F32;
             CU(linear(g)); ++nl;
         }
         CU(rmsnorm_rows_launch(pf_x_, L.ffn_norm, T, TP, n_embd_, eps_, pf_xn_, bf, s)); ++nl;
         {
             GemmParams g{};
-            g.a = pf_xn_; g.b = L.wgu16; g.c = pf_h_; g.m = T; g.n = 2 * n_ff_; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = n_ff_;
+            ST(prompt_operand(L, OP_GU, &g.b, &nl));
+            g.a = pf_xn_; g.c = pf_h_; g.m = T; g.n = 2 * n_ff_; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = n_ff_;
             g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_SILU;
             CU(linear(g)); ++nl;
         }
         {
             GemmParams g{};
-            g.a = pf_h_; g.b = L.wd16; g.c = pf_x_; g.m = T; g.n = n_embd_; g.k = n_ff_; g.lda = n_ff_; g.ldb = n_ff_; g.ldc = n_embd_;
+            ST(prompt_operand(L, OP_DOWN, &g.b, &nl));
+            g.a = pf_h_; g.c = pf_x_; g.m = T; g.n = n_embd_; g.k = n_ff_; g.lda = n_ff_; g.ldb = n_ff_; g.ldc = n_embd_;
             g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_ADD_F32;
             CU(linear(g)); ++nl;
         }
@@ -223,7 +259,8 @@ Status Engine::prefill_packed(const std::vector<int>& starts, const std::vector<
         bool roped = false;
         {
             GemmParams g{};
-            g.a = pf_xn_; g.b = L.wqkv16; g.c = pf_qkv_; g.m = TP; g.n = ldq; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = ldq;
+            ST(prompt_operand(L, OP_QKV, &g.b, &nl));
+            g.a = pf_xn_; g.c = pf_qkv_; g.m = TP; g.n = ldq; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = ldq;
             g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_F32;
             RopeSplitArgs ra{rope_cos_, rope_sin_, pf_q_, pf_k_, pf_vt_, kc, vc, n_head_, n_kv_, hd_, tp, {}};
             if (prefill_flash_ && prefill_fuse_rope_ && prefill_tc5_ && starts.size() <= (size_t)PF_MAX_SEGS) {
@@ -288,20 +325,23 @@ Status Engine::prefill_packed(const std::vector<int>& starts, const std::vector<
         }
         {
             GemmParams g{};
-            g.a = pf_attn_; g.b = L.wo16; g.c = pf_x_; g.m = TP; g.n = n_embd_; g.k = qd; g.lda = qd; g.ldb = qd; g.ldc = n_embd_;
+            ST(prompt_operand(L, OP_O, &g.b, &nl));
+            g.a = pf_attn_; g.c = pf_x_; g.m = TP; g.n = n_embd_; g.k = qd; g.lda = qd; g.ldb = qd; g.ldc = n_embd_;
             g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_ADD_F32;
             CU(linear(g)); ++nl;
         }
         CU(rmsnorm_rows_launch(pf_x_, L.ffn_norm, TP, TP, n_embd_, eps_, pf_xn_, bf, s)); ++nl;
         {
             GemmParams g{};
-            g.a = pf_xn_; g.b = L.wgu16; g.c = pf_h_; g.m = TP; g.n = 2 * n_ff_; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = n_ff_;
+            ST(prompt_operand(L, OP_GU, &g.b, &nl));
+            g.a = pf_xn_; g.c = pf_h_; g.m = TP; g.n = 2 * n_ff_; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = n_ff_;
             g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_SILU;
             CU(linear(g)); ++nl;
         }
         {
             GemmParams g{};
-            g.a = pf_h_; g.b = L.wd16; g.c = pf_x_; g.m = TP; g.n = n_embd_; g.k = n_ff_; g.lda = n_ff_; g.ldb = n_ff_; g.ldc = n_embd_;
+            ST(prompt_operand(L, OP_DOWN, &g.b, &nl));
+            g.a = pf_h_; g.c = pf_x_; g.m = TP; g.n = n_embd_; g.k = n_ff_; g.lda = n_ff_; g.ldb = n_ff_; g.ldc = n_embd_;
             g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_ADD_F32;
             CU(linear(g)); ++nl;
         }

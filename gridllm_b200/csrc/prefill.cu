@@ -8,11 +8,13 @@
 // The general GEMM: a TN GEMM  C[M x N] = A[M x K] * B[N x K]^T  on 16-bit inputs with fp32 accumulation
 // (mma.sync m16n8k16; the plain linear layers run on the TMA + wgmma kernel of prefill_tc5.cu), cp.async
 // 3-stage pipeline, XOR-swizzled shared memory, ldmatrix fragments, fused epilogues (residual add,
-// SiLU*mul).  Weights are dequantised once at load into a resident 16-bit copy (HBM is 80 GB; 16 GB for
-// Llama-3-8B).  Attention over the prompt is two batched GEMMs
+// SiLU*mul).  Weights are dequantised into 16-bit operands from the engine layouts: once at load into a resident
+// copy (14 GB for Llama-3-8B), or layer by layer into one staging buffer when that copy cannot fit (prefill_weights.h).  Attention over the prompt is two batched GEMMs
 // (Q K^T, P V) around a causal softmax.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+
+#include <algorithm>
 
 #include "common.cuh"
 #include "gguf_file.h"
@@ -24,18 +26,12 @@ namespace gl {
 
 namespace {
 
-// ---------------------------------------------------------------------------------------------
-// element access into ENGINE row layouts (rowdot.h) -- used once at load to build the 16-bit copy
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float dequant_engine(const uint8_t* mat, int type, int cols, int row_stride, int tile_rows, int r, int c) {
-    const uint8_t* row = mat + (size_t)r * row_stride;      // fp types: plain row-major
+// element c of a plain F32 / F16 / BF16 row
+__device__ __forceinline__ float dequant_fp_row(const uint8_t* row, int type, int c) {
     switch (type) {
         case T_F32: return reinterpret_cast<const float*>(row)[c];
         case T_F16: return __half2float(reinterpret_cast<const __half*>(row)[c]);
         case T_BF16: return __uint_as_float((uint32_t)reinterpret_cast<const uint16_t*>(row)[c] << 16);
-        case T_Q4_K:
-        case T_Q6_K:
-        case T_Q8_0: return dequant_engine_quant(mat, type, cols, tile_rows, r, c);
         default: return 0.f;
     }
 }
@@ -43,18 +39,6 @@ __device__ __forceinline__ float dequant_engine(const uint8_t* mat, int type, in
 template <typename T> __device__ __forceinline__ T from_float(float v);
 template <> __device__ __forceinline__ __half from_float<__half>(float v) { return __float2half_rn(v); }
 template <> __device__ __forceinline__ __nv_bfloat16 from_float<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
-
-template <typename T>
-__global__ void __launch_bounds__(256) dequant_rows_kernel(const uint8_t* __restrict__ src, int type, int rows, int cols, int row_stride, int tile_rows,
-                                                           T* __restrict__ dst, int dst_ld, int dst_row0, int interleave) {
-    for (int r = blockIdx.x; r < rows; r += gridDim.x) {
-        int dr = r;
-        if (interleave == 1) dr = (r >> 3) * 16 + (r & 7);            // gate rows
-        else if (interleave == 2) dr = (r >> 3) * 16 + 8 + (r & 7);   // up rows
-        T* out = dst + (size_t)(dst_row0 + dr) * dst_ld;
-        for (int c = threadIdx.x; c < cols; c += blockDim.x) out[c] = from_float<T>(dequant_engine(src, type, cols, row_stride, tile_rows, r, c));
-    }
-}
 
 // ---------------------------------------------------------------------------------------------
 // TN GEMM on mma.sync
@@ -331,7 +315,7 @@ __device__ __forceinline__ float dequant_native_row(const uint8_t* row, int type
         return half_bits_to_float(*reinterpret_cast<const uint16_t*>(b)) * (float)(int8_t)b[2 + (c & 31)];
     }
     if (type == T_Q4_K) return dequant_native_q4k(row, c);
-    return dequant_engine(row, type, 0, 0, 1, 0, c);     // F32 / F16 / BF16: plain rows
+    return dequant_fp_row(row, type, c);
 }
 
 __global__ void __launch_bounds__(256) embed_rows_kernel(const uint8_t* __restrict__ w, int type, int cols, int row_bytes, const int* __restrict__ ids,
@@ -340,6 +324,131 @@ __global__ void __launch_bounds__(256) embed_rows_kernel(const uint8_t* __restri
     if (t >= t_rows) return;
     const uint8_t* row = w + (size_t)ids[t] * row_bytes;
     for (int c = threadIdx.x; c < cols; c += 256) x[(size_t)t * cols + c] = dequant_native_row(row, type, c);
+}
+
+// ---------------------------------------------------------------------------------------------
+// 16-bit GEMM operands from the engine layouts (rowdot.h): the resident copy at load, the lm_head copy of the batched step and
+// the streamed prompt pass's staging buffer before every linear GEMM.  A quantised source is read one (row tile, K-segment)
+// range at a time -- one contiguous run of tile_rows * seg_bytes bytes, copied to shared memory with 16-byte cp.async -- and
+// every thread then writes 8 consecutive columns of one row as one 16-byte store.  The per-weight arithmetic is the GGUF
+// dequantisation in fp32 with its roundings spelled out (Q4_K: d*sc*q - dmin*m as one FMA after the two products; Q6_K:
+// (d*sc)*q; Q8_0: d*q), then one rounding to the 16-bit type, so the copy does not depend on how the compiler contracts.
+// ---------------------------------------------------------------------------------------------
+constexpr int DQ_THREADS = 256;
+constexpr int DQ_RANGE_MAX = 4 * MAX_KSEG_BLOCKS * 144;       // the largest range: a Q4_K tile of 4 rows x 16 blocks (9 KB)
+constexpr int DQ_FP_COLS = DQ_THREADS * 8;                    // columns of one item of a plain F32 / F16 / BF16 row
+
+struct DequantSrcDev {
+    DequantSrc s;
+    int nks, seg_nb, seg_bytes;    // quantised: the row geometry (ksplit); fp: nks = row pieces of DQ_FP_COLS columns
+    int item_end;                  // items of this and every earlier source
+};
+struct DequantParams {
+    DequantSrcDev src[DEQUANT_MAX_SRCS];
+    int n_src, cols, items;
+    void* dst;
+};
+
+// 8 columns [lc, lc + 8) of one engine segment (lc % 8 == 0); n = units per segment
+__device__ __forceinline__ void dq8_q4k(const uint8_t* seg, int lc, float* v) {
+    const uint8_t* b = seg + (lc >> 8) * 144;       // a Q4_K segment is a run of native super-blocks
+    const int e = lc & 255, sub = e >> 5, l = e & 31;
+    const float d = half_bits_to_float(*reinterpret_cast<const uint16_t*>(b));
+    const float dmin = half_bits_to_float(*reinterpret_cast<const uint16_t*>(b + 2));
+    const uint8_t* sc = b + 4;
+    int s, m;
+    if (sub < 4) { s = sc[sub] & 63; m = sc[4 + sub] & 63; }
+    else { s = (sc[4 + sub] & 0xF) | ((sc[sub - 4] >> 6) << 4); m = (sc[4 + sub] >> 4) | ((sc[sub] >> 6) << 4); }
+    const float ds = __fmul_rn(d, (float)s), dm = __fmul_rn(dmin, (float)m);
+    const uint2 q = *reinterpret_cast<const uint2*>(b + 16 + (sub >> 1) * 32 + l);
+    const int sh = (sub & 1) * 4;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const uint32_t w = k < 4 ? q.x : q.y;
+        v[k] = __fmaf_rn(ds, (float)((w >> (8 * (k & 3) + sh)) & 0xF), -dm);
+    }
+}
+
+__device__ __forceinline__ void dq8_q6k(const uint8_t* seg, int n, int lc, float* v) {
+    const int u = lc >> 7, w = lc & 127, i = w & 63, s = w >> 6, j = w & 31, t = w >> 5;
+    const uint2 ql = *reinterpret_cast<const uint2*>(seg + ((size_t)(i >> 4) * n + u) * 16 + (i & 15));
+    const uint2 qh = *reinterpret_cast<const uint2*>(seg + (size_t)n * 64 + ((size_t)(j >> 4) * n + u) * 16 + (j & 15));
+    const float d = half_bits_to_float(*reinterpret_cast<const uint16_t*>(seg + (size_t)n * 104 + (size_t)(u >> 1) * 2));
+    const float dsc = __fmul_rn(d, (float)(int8_t)seg[(size_t)n * 96 + (size_t)u * 8 + (w >> 4)]);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const int qlv = (((k < 4 ? ql.x : ql.y) >> (8 * (k & 3))) >> (4 * s)) & 0xF;
+        const int qhv = (((k < 4 ? qh.x : qh.y) >> (8 * (k & 3))) >> (2 * t)) & 3;
+        v[k] = __fmul_rn(dsc, (float)((qlv | (qhv << 4)) - 32));
+    }
+}
+
+__device__ __forceinline__ void dq8_q80(const uint8_t* seg, int n, int lc, float* v) {
+    const int u = lc >> 7, w = lc & 127;
+    const float d = half_bits_to_float(*reinterpret_cast<const uint16_t*>(seg + (size_t)n * 128 + (size_t)u * 8 + 2 * (w >> 5)));
+    const uint2 q = *reinterpret_cast<const uint2*>(seg + ((size_t)(w >> 4) * n + u) * 16 + (w & 15));
+#pragma unroll
+    for (int k = 0; k < 8; ++k) v[k] = __fmul_rn(d, (float)(int8_t)((k < 4 ? q.x : q.y) >> (8 * (k & 3))));
+}
+
+template <typename T>
+__device__ __forceinline__ void store8(T* out, const float* v) {
+    union { T h[8]; uint4 u; } pk;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) pk.h[k] = from_float<T>(v[k]);
+    *reinterpret_cast<uint4*>(out) = pk.u;
+}
+
+// destination row of source row r: gate / up rows interleave in groups of 8 (GEMM_EPI_SILU)
+__device__ __forceinline__ int dq_dst_row(const DequantSrc& s, int r) {
+    if (s.interleave == 1) return s.dst_row0 + (r >> 3) * 16 + (r & 7);
+    if (s.interleave == 2) return s.dst_row0 + (r >> 3) * 16 + 8 + (r & 7);
+    return s.dst_row0 + r;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(DQ_THREADS, 4) dequant_operand_kernel(const __grid_constant__ DequantParams p) {
+    __shared__ __align__(16) uint8_t sm[DQ_RANGE_MAX];
+    const int tid = threadIdx.x;
+    T* dst = reinterpret_cast<T*>(p.dst);
+    for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
+        int si = 0;
+        while (it >= p.src[si].item_end) ++si;
+        const DequantSrcDev& S = p.src[si];
+        const int li = it - (si ? p.src[si - 1].item_end : 0);
+        const int type = S.s.type;
+        if (type == T_Q4_K || type == T_Q6_K || type == T_Q8_0) {
+            const int tr = S.s.tile_rows, tile = li / S.nks, ks = li - tile * S.nks;
+            const int nbytes = tr * S.seg_bytes;
+            const uint8_t* g = S.s.w + engine_seg_offset(S.seg_bytes, S.nks, tr, tile * tr, ks);      // [tile][ks][row][seg]: contiguous
+            __syncthreads();                                 // the previous range's readers are done
+            const uint32_t sb = smem_u32(sm);
+            for (int i = tid; i < nbytes / 16; i += DQ_THREADS) cp_async16(sb + i * 16, g + (size_t)i * 16, true);
+            cp_async_commit();
+            cp_async_wait<0>();
+            __syncthreads();
+            const int seg_chunks = S.seg_nb * 32, n = 2 * S.seg_nb;
+            for (int j = tid; j < tr * seg_chunks; j += DQ_THREADS) {
+                const int rr = j / seg_chunks, lc = (j - rr * seg_chunks) * 8, r = tile * tr + rr;
+                if (r >= S.s.rows) break;                    // the padding rows of the last tile
+                const uint8_t* seg = sm + rr * S.seg_bytes;
+                float v[8];
+                if (type == T_Q4_K) dq8_q4k(seg, lc, v);
+                else if (type == T_Q6_K) dq8_q6k(seg, n, lc, v);
+                else dq8_q80(seg, n, lc, v);
+                store8<T>(dst + (size_t)dq_dst_row(S.s, r) * p.cols + (size_t)ks * S.seg_nb * 256 + lc, v);
+            }
+        } else {
+            const int r = li / S.nks, c = (li - r * S.nks) * DQ_FP_COLS + tid * 8;
+            if (c < p.cols) {
+                const uint8_t* row = S.s.w + (size_t)r * S.s.row_stride;
+                float v[8];
+#pragma unroll
+                for (int k = 0; k < 8; ++k) v[k] = dequant_fp_row(row, type, c + k);
+                store8<T>(dst + (size_t)dq_dst_row(S.s, r) * p.cols + c, v);
+            }
+        }
+    }
 }
 
 template <typename T, int EPI>
@@ -382,11 +491,37 @@ cudaError_t gemm_tn_launch(const GemmParams& p, bool bf16, cudaStream_t s) {
     return bf16 ? gemm_launch_d<__nv_bfloat16>(p, s) : gemm_launch_d<__half>(p, s);
 }
 
-cudaError_t dequant_rows_launch(const uint8_t* src, int type, int rows, int cols, int row_stride, int tile_rows, void* dst, int dst_ld, int dst_row0,
-                                int interleave, bool bf16, cudaStream_t s) {
-    const int blocks = rows < 132 * 8 ? rows : 132 * 8;
-    if (bf16) dequant_rows_kernel<__nv_bfloat16><<<blocks, 256, 0, s>>>(src, type, rows, cols, row_stride, tile_rows, (__nv_bfloat16*)dst, dst_ld, dst_row0, interleave);
-    else dequant_rows_kernel<__half><<<blocks, 256, 0, s>>>(src, type, rows, cols, row_stride, tile_rows, (__half*)dst, dst_ld, dst_row0, interleave);
+cudaError_t dequant_launch(const DequantOp& op, bool bf16, cudaStream_t s) {
+    if (op.n_src < 1 || op.n_src > DEQUANT_MAX_SRCS || op.cols <= 0 || op.cols % 8 || !op.dst) return cudaErrorInvalidValue;
+    DequantParams p{};
+    p.n_src = op.n_src; p.cols = op.cols; p.dst = op.dst;
+    long long items = 0;
+    for (int i = 0; i < op.n_src; ++i) {
+        DequantSrcDev& d = p.src[i];
+        d.s = op.src[i];
+        const int t = d.s.type;
+        if (t == T_Q4_K || t == T_Q6_K || t == T_Q8_0) {
+            const KSplit k = ksplit(op.cols);
+            if (!k.nks || d.s.tile_rows < 1) return cudaErrorInvalidValue;
+            d.nks = k.nks; d.seg_nb = k.seg_nb; d.seg_bytes = kseg_bytes(t, k.seg_nb);
+            if (d.s.tile_rows * d.seg_bytes > DQ_RANGE_MAX) return cudaErrorInvalidValue;
+            items += (long long)((d.s.rows + d.s.tile_rows - 1) / d.s.tile_rows) * d.nks;
+        } else if (t == T_F32 || t == T_F16 || t == T_BF16) {
+            if (d.s.row_stride % 16) return cudaErrorInvalidValue;
+            d.nks = (op.cols + DQ_FP_COLS - 1) / DQ_FP_COLS;
+            items += (long long)d.s.rows * d.nks;
+        } else {
+            return cudaErrorInvalidValue;
+        }
+        if (items > INT32_MAX) return cudaErrorInvalidValue;
+        d.item_end = (int)items;
+    }
+    p.items = (int)items;
+    if (!p.items) return cudaSuccess;
+    static const int sms = []() { int dev = 0, n = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); return n; }();
+    const int blocks = (int)std::min<long long>(p.items, (long long)sms * 4);
+    if (bf16) dequant_operand_kernel<__nv_bfloat16><<<blocks, DQ_THREADS, 0, s>>>(p);
+    else dequant_operand_kernel<__half><<<blocks, DQ_THREADS, 0, s>>>(p);
     return cudaGetLastError();
 }
 

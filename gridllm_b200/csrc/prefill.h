@@ -62,8 +62,23 @@ cudaError_t gemm_tn_launch(const GemmParams& p, bool bf16, cudaStream_t s);     
 cudaError_t gemm_tc5_configure();
 bool gemm_tc5_supported(const GemmParams& p);
 cudaError_t gemm_tc5_launch(const GemmParams& p, int a_rows_alloc, bool bf16, cudaStream_t s);
-cudaError_t dequant_rows_launch(const uint8_t* src, int type, int rows, int cols, int row_stride, int tile_rows, void* dst, int dst_ld, int dst_row0,
-                                int interleave, bool bf16, cudaStream_t s);
+// One source matrix of a 16-bit GEMM operand: engine layout (rowdot.h) for Q4_K / Q6_K / Q8_0, plain rows of row_stride bytes
+// (a multiple of 16) for F32 / F16 / BF16.  Its rows land at dst_row0 + r, or interleaved in groups of 8 as GEMM_EPI_SILU reads them.
+struct DequantSrc {
+    const uint8_t* w;
+    int type, rows, row_stride, tile_rows;
+    int dst_row0;
+    int interleave;     // 0: plain; 1: gate rows, 2: up rows of a [8 gate | 8 up] matrix (row r -> (r / 8) * 16 + (0 | 8) + r % 8)
+};
+constexpr int DEQUANT_MAX_SRCS = 3;
+struct DequantOp {
+    DequantSrc src[DEQUANT_MAX_SRCS];
+    int n_src;
+    int cols;           // columns of every source = row length of dst (a multiple of 8)
+    void* dst;          // [rows][cols] fp16 or bf16
+};
+// one launch dequantises every source of op (Q | K | V, gate / up, or a single matrix)
+cudaError_t dequant_launch(const DequantOp& op, bool bf16, cudaStream_t s);
 cudaError_t rmsnorm_rows_launch(const float* x, const float* w, int rows, int rows_pad, int n, float eps, void* y, bool bf16, cudaStream_t s);
 cudaError_t rope_split_launch(const float* qkv, int t_rows, int t_pad, int pos0, int n_head, int n_kv, int hd, const float* cos_t,
                               const float* sin_t, __half* qo, __half* ko, __half* vt, __half* k_cache, __half* v_cache,

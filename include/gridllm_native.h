@@ -53,7 +53,14 @@ typedef struct gl_engine_opts {
     int32_t act_bits;         /* GEMV activation fixed point: 16 (default, 2x int8 planes) or 8 (ggml-like) */
     int32_t use_graph;        /* 1 (default): decode step replayed as a CUDA graph; 0: plain launches */
     int32_t use_pdl;          /* 1 (default): programmatic dependent launch between step kernels */
-    int32_t prefill_mode;     /* 0 auto, 1 sequential decode steps, 2 batched tensor-core prefill */
+    int32_t prefill_mode;     /* 0 auto, 1 sequential decode steps, 2 batched tensor-core prefill.
+                                 The prompt pass's 16-bit layer matrices: resident (a copy of every layer matrix built at load, 2 bytes
+                                 per weight) when copy + 4 GB fits in the HBM free after the weights and the KV pool, else streamed
+                                 (each layer's four GEMM operands dequantised into one staging buffer, the size of the largest
+                                 operand, just before their GEMMs: 4 more launches per layer per pass; a 70B q4 model on one
+                                 80 GB H100).  Environment GL_PREFILL_WEIGHTS: 0 auto (default), 1 resident (the load fails with
+                                 GL_ERR_NOMEM when it does not fit), 2 streamed.  Under prefill_mode 1 neither is built.
+                                 Continuous batching (gl_seq_open*) needs the resident copy. */
     int32_t max_batch;        /* continuous batching: sequences that may be open at once (gl_seq_open); 0 / 1 = none, <= 128.
                                  The KV pool is provisioned for max_batch sequences of max_ctx tokens unless kv_pool_tokens says otherwise */
     int32_t kv_pool_tokens;   /* tokens of KV cache shared by all open sequences; 0 = max_ctx * max(1, max_batch) */
@@ -234,7 +241,9 @@ int  gl_chat_template(const gl_engine* e, char* buf, int32_t cap, int32_t* len_o
 int  gl_generate(gl_engine* e, const int32_t* prompt, int32_t n_prompt, const gl_sample_opts* opts,
                  gl_token_cb cb, void* user, int32_t* out_ids, float* out_logprobs, gl_gen_stats* stats);
 /* gl_embed: generateEmbedding (OllamaService.ts:601-665): prefill only, output_norm, mean-pool,
- *   L2-normalise. seq_offsets has n_seq+1 entries into ids. out is [n_seq][n_embd]. */
+ *   L2-normalise. seq_offsets has n_seq+1 entries into ids. out is [n_seq][n_embd].  Sequences are packed into tensor-core prompt
+ *   passes whichever source the pass reads its weights from (resident or streamed, gl_engine_opts prefill_mode); a sequence longer
+ *   than 2 048 tokens takes passes of its own.  Under prefill_mode 1 every sequence steps through the decode kernels. */
 int  gl_embed(gl_engine* e, const int32_t* ids, const int32_t* seq_offsets, int32_t n_seq,
               float* out, gl_gen_stats* stats);
 /* ---- continuous batching inside one engine (SURVEY.md section 8f.1) ----------------------------------------------------
@@ -362,7 +371,8 @@ int  gl_position(const gl_engine* e, int32_t* pos);
 /* batched prefill of n tokens from the current position; logits of the LAST token (may be NULL).  Like gl_generate, gl_seq_open
  * and gl_embed, it takes the tensor-core prompt pass at any length up to the engine's context (passes of 4 096 rows; a pass that
  * does not start at position 0 attends to the earlier positions through the KV pages), and a prompt prefilled in pieces gives
- * the bits of the same prompt in one call.  Under prefill_mode 1, or fewer than 8 tokens, the tokens step through the decode kernels. */
+ * the bits of the same prompt in one call.  The pass reads the resident 16-bit copy or streams the layer matrices (gl_engine_opts
+ * prefill_mode); both give the same bits.  Under prefill_mode 1, or fewer than 8 tokens, the tokens step through the decode kernels. */
 int  gl_prefill(gl_engine* e, const int32_t* ids, int32_t n, float* last_logits);
 /* mean device time (ms) of one decode step replayed `iters` times at context length ctx_len
  * (KV content is whatever is resident; used for the roofline line) */
