@@ -346,6 +346,15 @@ __global__ void __launch_bounds__(128, 2) batch_attn_mma_kernel(const __grid_con
             }
             __syncwarp();
         }
+        if (npos < KV_PAGE_TOKENS) {
+            // the row's last page: its slots past the position belong to no one yet -- a page back from the pool still holds its
+            // previous owner's rows, which may be inf.  P = 0 there, but 0 * inf = NaN in P V: zero those V rows (whole rows, so
+            // the swizzle does not matter).
+            const uint32_t z0 = vb + (uint32_t)(npos * Cfg::ROW_BYTES);
+            for (int i = lane; i < (KV_PAGE_TOKENS - npos) * Cfg::CHUNKS_PER_ROW; i += 32)
+                asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(z0 + (uint32_t)i * 16), "r"(0u) : "memory");
+            __syncwarp();
+        }
         // ---- S = Q K^T : two n-tiles (positions 0-7, 8-15) ----
         float s0[4] = {0.f, 0.f, 0.f, 0.f}, s1[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
@@ -365,7 +374,8 @@ __global__ void __launch_bounds__(128, 2) batch_attn_mma_kernel(const __grid_con
         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
         const float m_new = fmaxf(m_run, mx);                       // npos >= 1: finite
         const float corr = (m_run == -INFINITY) ? 0.f : expf(m_run - m_new);
-        const float p0 = expf(v0 - m_new), p1 = expf(v1 - m_new), p2 = expf(v2 - m_new), p3 = expf(v3 - m_new);      // exp(-inf) = 0
+        // exp(-inf) = 0: positions past npos get P = 0, and their V rows were zeroed above
+        const float p0 = expf(v0 - m_new), p1 = expf(v1 - m_new), p2 = expf(v2 - m_new), p3 = expf(v3 - m_new);
         float ps = (p0 + p1) + (p2 + p3);
         ps += __shfl_xor_sync(0xffffffffu, ps, 1);
         ps += __shfl_xor_sync(0xffffffffu, ps, 2);
