@@ -534,51 +534,13 @@ Status Engine::set_state(int pos, int token, int n_prompt, int out_idx, const gl
 // decode step
 // -------------------------------------------------------------------------------------------------
 Status Engine::enqueue_gemv(cudaStream_t s, GemvParams& p, const GemvMat* mats, int nmat, bool pair, int cols, int* n_launch) {
-    // slot size: what the widest item of this kernel needs (Q4_K: 4 row segments, Q6_K / Q8_0: 2), ring depth: whatever
-    // shared memory is left, capped so that the bytes in flight stay near what the HBM pipe needs
-    int need = 0;
-    {
-        const KSplit ks = ksplit(cols);
-        if (!ks.nks) return fail(GL_ERR_UNSUPPORTED, "GEMV shape outside the kernel envelope (cols=" + std::to_string(cols) + ")");
-        for (int i = 0; i < nmat; ++i) need = std::max(need, item_rows(mats[i].type) * kseg_bytes(mats[i].type, ks.seg_nb));
-    }
-    p.slot_bytes = (need + 127) & ~127;
-    if (!gemv_plan(p, mats, nmat, pair, cols, p.slot_bytes)) return fail(GL_ERR_UNSUPPORTED, "GEMV shape outside the kernel envelope (cols=" + std::to_string(cols) + ")");
-    // prologue variant (= which kernel, gemv.cu): by default the 256-bit-load half-block prologue for every width, so that all
-    // GEMV launches of a step are one kernel; GL_XRAW=1 stages narrow rows raw by one bulk copy instead (16 KB of ring)
-    p.xraw_bytes = 0;
-    p.xraw_nseg = 1;
-    const bool variants = gemv_prologue_variants(nw_);
-    p.hb256 = (variants && hb256_ && (cols > GEMV_XRAW_MAX_COLS || !xraw_) && cols <= 16 * nw_ * 32 * (nw_ >= 12 ? 3 : 4)) ? 1 : 0;
-    if (variants && xraw_ && !p.hb256) {
-        const KSplit ks = ksplit(cols);
-        if (cols <= GEMV_XRAW_MAX_COLS && cols / 16 <= nw_ * 32) {
-            p.xraw_bytes = cols * 4;
-        } else if (xraw_wide_ && ks.nks > 1 && cols / ks.nks / 16 <= nw_ * 32) {     // wide rows: K-segment pieces, two buffers
-            p.xraw_nseg = ks.nks;
-            p.xraw_bytes = 2 * (cols / ks.nks) * 4;
-        }
-    }
-    const size_t fixed = gemv_smem_bytes(cols, 0, 0) + (size_t)p.xraw_bytes;
-    const int ns = std::min(RING_MAX_SLOTS, (int)(((size_t)smem_kb_ * 1024 - fixed) / p.slot_bytes));
-    // as many consumer warps as there are, each with >= 2 slots; spare slots deepen the tracks (small slots: more bytes in flight)
-    // tracks x depth: as many bytes in flight as the ring can hold, giving up at most two consumer warps for depth
-    // (small slots -- Q6_K pairs -- would otherwise leave a third of the shared memory unused: lm_head 0.94 -> 0.86 of peak)
-    p.n_tracks = std::min(nw_, ns / 2);
-    p.depth = p.n_tracks > 0 ? std::min(ring_depth_max_, ns / p.n_tracks) : 0;
-    for (int t = std::max(1, nw_ - 2); p.pd.nks > 1 && t < std::min(nw_, ns / 2); ++t) {      // (narrow rows keep every warp: lm_head is issue-bound at 10)
-        const int dd = std::min(ring_depth_max_, ns / t);
-        if (dd >= 2 && t * dd > p.n_tracks * p.depth) { p.n_tracks = t; p.depth = dd; }
-    }
-    // a phase in which no warp gets a second slot (one round of items, one K-segment) needs one slot per warp: the smaller
-    // footprint (121 KB instead of 232 KB) lets the next kernel's CTAs become resident -- and start their own prefetch --
-    // while this one is still running (programmatic dependent launch)
-    if (lean_rings_ && p.n_tracks > 0 && p.pd.nks == 1) {
-        int items = 0;
-        for (int i = 0; i < (pair ? 1 : nmat); ++i) items += p.pd.seg[i].n_items;
-        if ((items + sm_count_ - 1) / sm_count_ <= p.n_tracks) p.depth = 1;
-    }
-    if (p.n_tracks < 1) return fail(GL_ERR_UNSUPPORTED, "GEMV staging does not fit shared memory");
+    // slot bytes, prologue variant, tracks x depth and lean ring: gemv_geometry (gemv.cu), shared with the kernel tests
+    GemvGeomOpts o;
+    o.nw = nw_; o.smem_kb = smem_kb_; o.ring_depth_max = ring_depth_max_;
+    o.hb256 = hb256_; o.xraw = xraw_; o.xraw_wide = xraw_wide_; o.lean_rings = lean_rings_;
+    const int g = gemv_geometry(p, mats, nmat, pair, cols, o, sm_count_);
+    if (g == GEMV_GEOM_SHAPE) return fail(GL_ERR_UNSUPPORTED, "GEMV shape outside the kernel envelope (cols=" + std::to_string(cols) + ")");
+    if (g != GEMV_GEOM_OK) return fail(GL_ERR_UNSUPPORTED, "GEMV staging does not fit shared memory");
     p.trace = perop_trace_ ? perop_trace_ + 16 * (size_t)std::min(*n_launch, PEROP_TRACE_LAUNCHES - 1) : nullptr;
     CU(gemv_launch(p, abits_, nw_, sm_count_, use_pdl_, s));
     ++*n_launch;

@@ -144,6 +144,52 @@ bool gemv_plan(GemvParams& p, const GemvMat* mats, int nmat, bool pair, int cols
     return true;
 }
 
+int gemv_geometry(GemvParams& p, const GemvMat* mats, int nmat, bool pair, int cols, const GemvGeomOpts& o, int n_ctas) {
+    // slot size: what the widest item of this kernel needs (Q4_K: 4 row segments, Q6_K / Q8_0: 2), ring depth: whatever
+    // shared memory is left, capped so that the bytes in flight stay near what the HBM pipe needs
+    const KSplit ks = ksplit(cols);
+    if (!ks.nks || nmat < 1 || nmat > 3) return GEMV_GEOM_SHAPE;
+    int need = 0;
+    for (int i = 0; i < nmat; ++i) need = std::max(need, item_rows(mats[i].type) * kseg_bytes(mats[i].type, ks.seg_nb));
+    p.slot_bytes = (need + 127) & ~127;
+    if (!gemv_plan(p, mats, nmat, pair, cols, p.slot_bytes)) return GEMV_GEOM_SHAPE;
+    // prologue variant (= which kernel): by default the 256-bit-load half-block prologue for every width, so that all GEMV
+    // launches of a step are one kernel; xraw stages narrow rows raw by one bulk copy instead (16 KB of ring)
+    const int nw = o.nw;
+    p.xraw_bytes = 0;
+    p.xraw_nseg = 1;
+    const bool variants = gemv_prologue_variants(nw);
+    p.hb256 = (variants && o.hb256 && (cols > GEMV_XRAW_MAX_COLS || !o.xraw) && cols <= 16 * nw * 32 * (nw >= 12 ? 3 : 4)) ? 1 : 0;
+    if (variants && o.xraw && !p.hb256) {
+        if (cols <= GEMV_XRAW_MAX_COLS && cols / 16 <= nw * 32) {
+            p.xraw_bytes = cols * 4;
+        } else if (o.xraw_wide && ks.nks > 1 && cols / ks.nks / 16 <= nw * 32) {     // wide rows: K-segment pieces, two buffers
+            p.xraw_nseg = ks.nks;
+            p.xraw_bytes = 2 * (cols / ks.nks) * 4;
+        }
+    }
+    const size_t fixed = gemv_smem_bytes(cols, 0, 0) + (size_t)p.xraw_bytes;
+    const int ns = std::min(RING_MAX_SLOTS, (int)(((size_t)o.smem_kb * 1024 - fixed) / p.slot_bytes));
+    // as many consumer warps as there are, each with >= 2 slots; spare slots deepen the tracks (small slots: more bytes in flight)
+    // tracks x depth: as many bytes in flight as the ring can hold, giving up at most two consumer warps for depth
+    // (small slots -- Q6_K pairs -- would otherwise leave a third of the shared memory unused: lm_head 0.94 -> 0.86 of peak)
+    p.n_tracks = std::min(nw, ns / 2);
+    p.depth = p.n_tracks > 0 ? std::min(o.ring_depth_max, ns / p.n_tracks) : 0;
+    for (int t = std::max(1, nw - 2); p.pd.nks > 1 && t < std::min(nw, ns / 2); ++t) {      // (narrow rows keep every warp: lm_head is issue-bound at 10)
+        const int dd = std::min(o.ring_depth_max, ns / t);
+        if (dd >= 2 && t * dd > p.n_tracks * p.depth) { p.n_tracks = t; p.depth = dd; }
+    }
+    // a phase in which no warp gets a second slot (one round of items, one K-segment) needs one slot per warp: the smaller
+    // footprint (121 KB instead of 232 KB) lets the next kernel's CTAs become resident -- and start their own prefetch --
+    // while this one is still running (programmatic dependent launch)
+    if (o.lean_rings && p.n_tracks > 0 && p.pd.nks == 1) {
+        int items = 0;
+        for (int i = 0; i < (pair ? 1 : nmat); ++i) items += p.pd.seg[i].n_items;
+        if ((items + n_ctas - 1) / n_ctas <= p.n_tracks) p.depth = 1;
+    }
+    return p.n_tracks < 1 ? GEMV_GEOM_SMEM : GEMV_GEOM_OK;
+}
+
 bool gemv_variant_ok(int abits, int nw) { return (abits == 16 || abits == 8) && (nw == 8 || nw == 12 || nw == 16); }
 
 namespace {

@@ -82,6 +82,23 @@ size_t gemv_smem_bytes(int cols, int n_slots, int slot_bytes);
 // Fills p.pd (K-segmentation, rows per item, item counts) for nmat matrices sharing cols; slot_bytes is the ring's
 // slot size the items must fit.  Returns false if the shape is outside the kernel's envelope.
 bool gemv_plan(GemvParams& p, const GemvMat* mats, int nmat, bool pair, int cols, int slot_bytes);
+
+// The switches a stand-alone GEMV launch is staged by (engine.h members; GL_WARPS, GL_SMEM_KB, GL_RING_DEPTH_MAX, GL_HB256,
+// GL_XRAW, GL_XRAW_WIDE, GL_LEAN_RINGS).  The defaults are the engine's when no variable overrides them.
+struct GemvGeomOpts {
+    int nw = 12;               // consumer warps
+    int smem_kb = 227;         // dynamic shared memory a CTA may take
+    int ring_depth_max = 3;    // slots per track
+    bool hb256 = true;         // half-block prologue with 256-bit loads, every width it fits
+    bool xraw = false;         // narrow rows staged raw by one bulk copy
+    bool xraw_wide = false;    // wide rows staged raw by K-segment pieces
+    bool lean_rings = true;    // one slot per track for single-round, single-K-segment launches
+};
+enum GemvGeomResult : int { GEMV_GEOM_OK = 0, GEMV_GEOM_SHAPE = 1, GEMV_GEOM_SMEM = 2 };
+// Plans one launch (gemv_plan) and decides its ring geometry over n_ctas CTAs: slot bytes, the prologue variant (hb256,
+// xraw_bytes, xraw_nseg), n_tracks x depth and the lean ring.  GEMV_GEOM_SHAPE: the shape is outside the kernel's envelope;
+// GEMV_GEOM_SMEM: the staging does not fit shared memory.
+int gemv_geometry(GemvParams& p, const GemvMat* mats, int nmat, bool pair, int cols, const GemvGeomOpts& o, int n_ctas);
 cudaError_t gemv_configure();   // opt-in to large dynamic shared memory (once per process)
 bool gemv_prologue_variants(int consumer_warps);   // are the specialised prologues (raw staging, 256-bit loads) compiled for this width?
 cudaError_t gemv_launch(const GemvParams& p, int abits, int consumer_warps, int n_ctas, bool pdl, cudaStream_t s);
