@@ -1308,7 +1308,7 @@ Status Engine::prefill(const int32_t* ids, int n, float* last_logits) {
 // generateEmbedding (/root/reference/client/src/services/OllamaService.ts:601-665; the batched form is `input: string[]` of
 // /api/embed, server/src/routes/ollama.ts:574-643): prompt pass only -> output_norm -> mean over positions -> L2 normalise.
 // The sequences of a call are PACKED: up to EMB_PACK_TOKENS rows share one pass over the layers (engine_prefill.cu
-// prefill_packed), each sequence attending only to itself.  No allocation per call (buffers grow on demand and stay), the
+// prompt_pass), each sequence attending only to itself.  No allocation per call (buffers grow on demand and stay), the
 // device time in the stats is bracketed by events around device work only.
 Status Engine::embed(const int32_t* ids, const int32_t* offs, int n_seq, float* out, gl_gen_stats* stats) {
     CU(cudaSetDevice(device_));
@@ -1328,11 +1328,7 @@ Status Engine::embed(const int32_t* ids, const int32_t* offs, int n_seq, float* 
         if (e == cudaSuccess) allocs_.push_back(*p);
         return e;
     };
-    if (!pk_ids_) {
-        CU(dalloc((void**)&pk_ids_, (size_t)EMB_PACK_TOKENS * 4));
-        CU(dalloc((void**)&emb_pooled_, (size_t)n_embd_ * 4));
-        CU(dalloc((void**)&emb_rstd_, (size_t)std::max(EMB_PACK_TOKENS, n_ctx_) * 4));
-    }
+    ST(ensure_pack_buffers());
     if (n_seq > emb_out_cap_) {                            // grows, never shrinks; the old buffer stays in allocs_ until the engine goes
         CU(cudaStreamSynchronize(stream_));
         CU(dalloc((void**)&emb_out_, (size_t)n_seq * n_embd_ * 4));
@@ -1346,19 +1342,21 @@ Status Engine::embed(const int32_t* ids, const int32_t* offs, int n_seq, float* 
         int sidx = 0;
         std::vector<int32_t> h_ids(EMB_PACK_TOKENS);
         while (sidx < n_seq) {
-            std::vector<int> starts, lens, which;
+            std::vector<PromptSeq> seqs;
+            std::vector<int> which;
             int rows = 0;
             std::fill(h_ids.begin(), h_ids.end(), 0);
             while (sidx < n_seq) {
                 const int n = offs[sidx + 1] - offs[sidx], lp = (n + 127) / 128 * 128;
                 if (n > EMB_PACK_TOKENS) break;            // longer than a pack: handled alone below
                 if (rows + lp > EMB_PACK_TOKENS) break;
-                starts.push_back(rows); lens.push_back(n); which.push_back(sidx);
+                seqs.push_back({rows, n, 0, nullptr});
+                which.push_back(sidx);
                 std::memcpy(h_ids.data() + rows, ids + offs[sidx], (size_t)n * 4);
                 rows += lp;
                 ++sidx;
             }
-            if (starts.empty()) {                          // one sequence longer than a pack: the single-sequence batched pass
+            if (seqs.empty()) {                            // one sequence longer than a pack: the single-sequence batched pass
                 const int n = offs[sidx + 1] - offs[sidx];
                 ST(kv_reset());
                 ST(ensure_pages(n));
@@ -1376,7 +1374,7 @@ Status Engine::embed(const int32_t* ids, const int32_t* offs, int n_seq, float* 
                     // normalised columns of every pass, then scales and L2-normalises once
                     for (int c0 = 0; c0 < n; c0 += PF_CHUNK) {
                         const int len = std::min(PF_CHUNK, n - c0);
-                        ST(prefill_chunk(c0, len, &launches));
+                        ST(prompt_pass({{0, len, c0, page_table_}}, len, prompt_ids_ + c0, &launches));
                         CU(pool_embedding_sum_launch(pf_x_, len, n_embd_, eps_, emb_rstd_, emb_pooled_, c0 > 0, stream_));
                         launches += 2;
                     }
@@ -1387,9 +1385,9 @@ Status Engine::embed(const int32_t* ids, const int32_t* offs, int n_seq, float* 
                 continue;
             }
             CU(cudaMemcpyAsync(pk_ids_, h_ids.data(), (size_t)rows * 4, cudaMemcpyHostToDevice, stream_));      // pageable source: staged before return
-            ST(prefill_packed(starts, lens, rows, &launches));
-            for (size_t i = 0; i < starts.size(); ++i) {
-                CU(pool_embedding_launch(pf_x_ + (size_t)starts[i] * n_embd_, lens[i], n_embd_, output_norm_, eps_, emb_rstd_, emb_pooled_,
+            ST(prompt_pass(seqs, rows, pk_ids_, &launches));
+            for (size_t i = 0; i < seqs.size(); ++i) {
+                CU(pool_embedding_launch(pf_x_ + (size_t)seqs[i].start * n_embd_, seqs[i].len, n_embd_, output_norm_, eps_, emb_rstd_, emb_pooled_,
                                          emb_out_ + (size_t)which[i] * n_embd_, stream_));
                 launches += 3;
             }

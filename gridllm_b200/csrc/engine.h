@@ -127,14 +127,18 @@ private:
     Status ensure_prefill_scratch(int t_pad);
     // positions [pos0, pos0 + n) of the single sequence, tokens already in prompt_ids_[pos0 .. pos0 + n), in passes of <= PF_CHUNK rows
     Status prefill_batched(int pos0, int n, int* n_launch);
-    Status prefill_chunk(int pos0, int n, int* n_launch);
     static constexpr int PF_CHUNK = 4096;             // rows of one prompt pass (the prefill scratch never grows past it)
-    // embeddings: several sequences in ONE prompt pass (block-diagonal causal attention); seq s = rows [starts[s], starts[s] + lens[s])
-    // tables: per sequence, the device page table its K / V rows are cached through (null: nothing is cached -- embeddings);
-    // pos0: per sequence, the absolute position of its first row (null: all 0), earlier positions being in its pages already
-    Status prefill_packed(const std::vector<int>& starts, const std::vector<int>& lens, int t_rows, int* n_launch,
-                          const std::vector<const int*>* tables = nullptr, const std::vector<int>* pos0 = nullptr);
+    // one sequence of a prompt pass: rows [start, start + len) hold its positions [pos0, pos0 + len), earlier positions being in
+    // its pages already; table: the device page table its K / V rows are cached through (null: nothing is cached -- embeddings)
+    struct PromptSeq {
+        int start, len, pos0;
+        const int* table;
+    };
+    // ONE prompt pass over rows [0, t_rows) of the pf_* scratch, token ids ids[0 .. t_rows): the sequences share the linear layers
+    // and each attends only to itself (block-diagonal causal attention); hidden states end up in pf_x_
+    Status prompt_pass(const std::vector<PromptSeq>& seqs, int t_rows, const int* ids, int* n_launch);
     static constexpr int EMB_PACK_TOKENS = 2048;      // rows of one packed pass (each sequence starts on a 128-row boundary)
+    Status ensure_pack_buffers();                     // pk_ids_, emb_pooled_ and emb_rstd_, allocated on first use
     int* pk_ids_ = nullptr;                           // [EMB_PACK_TOKENS] token ids of a pack (pad rows: token 0)
     float *emb_out_ = nullptr, *emb_rstd_ = nullptr, *emb_pooled_ = nullptr;
     int emb_out_cap_ = 0;

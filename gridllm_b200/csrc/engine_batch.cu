@@ -362,7 +362,7 @@ Status Engine::seq_open_single(const int32_t* prompt, int n_prompt, const gl_sam
     return {};
 }
 
-// Several prompts at once: they share ONE packed prompt pass per <= EMB_PACK_TOKENS rows (engine_prefill.cu prefill_packed: the
+// Several prompts at once: they share ONE packed prompt pass per <= EMB_PACK_TOKENS rows (engine_prefill.cu prompt_pass: the
 // linear layers see all their tokens as one [T x n_embd] matrix, each sequence attends only to itself and caches its K / V rows
 // through its own page table), then one lm_head GEMM over the last hidden row of every sequence and one sampler pass draw all the
 // first tokens.  32 prompts of 512 tokens: 8 passes with M = 2048 instead of 32 passes with M = 512, and one 1 GB lm_head read
@@ -406,16 +406,7 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
         ids = cut_ids.data();
         offs = cut_offs.data();
     }
-    if (!pk_ids_) {
-        auto dalloc = [&](void** p, size_t bytes) -> cudaError_t {
-            cudaError_t e = cudaMalloc(p, bytes);
-            if (e == cudaSuccess) allocs_.push_back(*p);
-            return e;
-        };
-        CU(dalloc((void**)&pk_ids_, (size_t)EMB_PACK_TOKENS * 4));
-        CU(dalloc((void**)&emb_pooled_, (size_t)n_embd_ * 4));
-        CU(dalloc((void**)&emb_rstd_, (size_t)std::max(EMB_PACK_TOKENS, n_ctx_) * 4));
-    }
+    ST(ensure_pack_buffers());
     const bool packable = prefill_w_ == PREFILL_W_RESIDENT;
     const bool share = packable && share_prefixes();
     const int64_t t_open = std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now().time_since_epoch()).count();
@@ -423,8 +414,8 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
     std::vector<int32_t> h_ids(EMB_PACK_TOKENS);
     while (next < n_seq) {
         // ---- one pack: as many of the next prompts as fit EMB_PACK_TOKENS rows, free slots and free pages ----
-        std::vector<int> starts, lens, which, pslots, shared;
-        std::vector<const int*> tables;
+        std::vector<PromptSeq> seqs;
+        std::vector<int> which, pslots;
         std::vector<int> indexed;                    // pages this pack added to the prefix index (taken out again if its pass fails)
         int rows = 0;
         bool out_of_room = false;
@@ -454,8 +445,8 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             if (share_i) index_prompt_pages(prompt, n, S.pages, r / KV_PAGE_TOKENS, &indexed);
             const int len = n - r;
             std::memcpy(h_ids.data() + rows, prompt + r, (size_t)len * 4);
-            starts.push_back(rows); lens.push_back(len); which.push_back(next); pslots.push_back(slot); shared.push_back(r);
-            tables.push_back(btables_ + (size_t)slot * n_pages_);
+            seqs.push_back({rows, len, r, btables_ + (size_t)slot * n_pages_});
+            which.push_back(next); pslots.push_back(slot);
             rows += (len + 127) / 128 * 128;
             ++next;
         }
@@ -482,11 +473,11 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             cudaError_t ce = cudaMemcpyAsync(pk_ids_, h_ids.data(), (size_t)rows * 4, cudaMemcpyHostToDevice, stream_);
             if (ce == cudaSuccess) ce = cudaEventRecord(ev_[2], stream_);
             if (ce != cudaSuccess) { rs = failb(GL_ERR_CUDA, cudaGetErrorString(ce)); break; }
-            rs = prefill_packed(starts, lens, rows, &launches, &tables, &shared);
+            rs = prompt_pass(seqs, rows, pk_ids_, &launches);
             if (!rs.ok()) break;
             // first tokens: last hidden row of each sequence -> rows 0..P-1 of the batched-step buffers -> final norm -> lm_head GEMM
             for (int i = 0; i < P && ce == cudaSuccess; ++i)
-                ce = cudaMemcpyAsync(bx_ + (size_t)i * n_embd_, pf_x_ + (size_t)(starts[i] + lens[i] - 1) * n_embd_, (size_t)n_embd_ * 4,
+                ce = cudaMemcpyAsync(bx_ + (size_t)i * n_embd_, pf_x_ + (size_t)(seqs[i].start + seqs[i].len - 1) * n_embd_, (size_t)n_embd_ * 4,
                                      cudaMemcpyDeviceToDevice, stream_);
             if (ce == cudaSuccess) ce = batch_rmsnorm_launch(bx_, output_norm_, P, n_embd_, eps_, bxn16_, stream_);
             if (ce == cudaSuccess) {
@@ -502,7 +493,7 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             hc.n_rows = P;
             bool any_pen = false, any_mask = false;
             for (int i = 0; i < P && ce == cudaSuccess; ++i) {
-                const int w = which[i], n = lens[i] + shared[i];
+                const int w = which[i], n = seqs[i].len + seqs[i].pos0;
                 const DrawPlan& plan = plans[w];
                 hst[i] = make_state(n - 1, ids[offs[w] + n - 1], n, 0, &opts[w]);
                 slots_[pslots[i]].plan = plan;
@@ -554,13 +545,13 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             return rs;
         }
         int64_t pack_tokens = 0;
-        for (int i = 0; i < P; ++i) pack_tokens += lens[i];
+        for (int i = 0; i < P; ++i) pack_tokens += seqs[i].len;
         for (int i = 0; i < P; ++i) {
             SeqSlot& S = slots_[pslots[i]];
             const int w = which[i];
             S.open = true;
-            S.n_prompt = lens[i] + shared[i];
-            S.n_shared = shared[i];
+            S.n_prompt = seqs[i].len + seqs[i].pos0;
+            S.n_shared = seqs[i].pos0;
             S.n_pred = opts[w].num_predict > 0 ? opts[w].num_predict : 128;
             S.produced = 0;
             S.first_pending = true;
@@ -572,12 +563,12 @@ Status Engine::seq_open_many(const int32_t* ids, const int32_t* offs, int n_seq,
             S.done = ho[i].done != 0;
             S.stopped = S.done;
             S.t_open_ns = t_open;
-            S.prefill_ns = (int64_t)(pack_ms * 1e6 * (double)lens[i] / (double)pack_tokens);      // its share of the pass
+            S.prefill_ns = (int64_t)(pack_ms * 1e6 * (double)seqs[i].len / (double)pack_tokens);      // its share of the pass
             S.launches = launches / P;
             slots_out[w] = pslots[i];
-            bc_[4] += (uint64_t)lens[i];
+            bc_[4] += (uint64_t)seqs[i].len;
             bc_[5] += 1;
-            bc_[7] += (uint64_t)shared[i];
+            bc_[7] += (uint64_t)seqs[i].pos0;
         }
         bc_[3] += (uint64_t)(pack_ms * 1e6);
         bc_[6] += (uint64_t)launches;

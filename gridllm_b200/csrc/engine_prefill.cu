@@ -126,9 +126,7 @@ Status Engine::prefill_batched(int pos0, int n, int* n_launch) {
     int nl = 0;
     for (int c0 = 0; c0 < n; c0 += PF_CHUNK) {
         const int len = std::min(PF_CHUNK, n - c0);
-        int nc = 0;
-        ST(prefill_chunk(pos0 + c0, len, &nc));
-        nl += nc;
+        ST(prompt_pass({{0, len, pos0 + c0, page_table_}}, len, prompt_ids_ + pos0 + c0, &nl));
     }
     // hidden state of the last prompt token -> the decode path's x buffer (lm_head / sampler follow)
     const int last = (n - 1) % PF_CHUNK;
@@ -138,40 +136,54 @@ Status Engine::prefill_batched(int pos0, int n, int* n_launch) {
     return {};
 }
 
-// One pass of prefill_batched: positions [pos0, pos0 + n), n <= PF_CHUNK; hidden states end up in pf_x_ rows 0 .. n - 1
-Status Engine::prefill_chunk(int pos0, int n, int* n_launch) {
-    const int T = n, TP = (n + 127) / 128 * 128;
+// One pass over the layers for rows [0, t_rows) of the pf_* scratch.  The sequences share the linear layers -- one
+// [t_rows x n_embd] activation matrix, every weight matrix read once per pass -- and each attends only to itself
+// (block-diagonal causal attention), and to its positions before pos0 through its pages.  Two kinds of caller:
+// prefill_batched and gl_embed's sequences longer than a pack run one sequence {0, n, pos0, page_table_} with t_rows = n <=
+// PF_CHUNK; the packs of gl_embed and gl_seq_open_many start every sequence on a 128-row boundary and pass a 128-aligned
+// t_rows.  Rows t_rows .. TP - 1 are padding that nothing reads back.
+Status Engine::prompt_pass(const std::vector<PromptSeq>& seqs, int t_rows, const int* ids, int* n_launch) {
+    if (!prefill_flash_)
+        for (const PromptSeq& q : seqs)
+            if (q.pos0 > 0) return failp(GL_ERR_UNSUPPORTED, "a prompt pass from a non-zero position needs the fused prompt attention");
+    const int TP = (t_rows + 127) / 128 * 128;
     const int qd = n_head_ * hd_, kvd = n_kv_ * hd_, ldq = qd + 2 * kvd, grp = n_head_ / n_kv_;
-    if (pos0 > 0 && !prefill_flash_) return failp(GL_ERR_UNSUPPORTED, "a prompt pass from a non-zero position needs the fused prompt attention");
     ST(ensure_prefill_scratch(TP));
     const int tp = pf_cap_;          // leading dimension of the [T_pad]-shaped scratch
     cudaStream_t s = stream_;
     const bool bf = prefill_bf16_;
+    // gl_seq_open_many and the single sequence cache their K / V rows through their tables; embedding packs cache nothing
+    const bool cached = std::any_of(seqs.begin(), seqs.end(), [](const PromptSeq& q) { return q.table != nullptr; });
+    // one segment list per PF_MAX_SEGS sequences: one RoPE / split launch and one fused attention launch each
+    std::vector<PrefillSegs> groups((seqs.size() + PF_MAX_SEGS - 1) / PF_MAX_SEGS, PrefillSegs{});
+    for (size_t i = 0; i < seqs.size(); ++i) {
+        PrefillSegs& g = groups[i / PF_MAX_SEGS];
+        g.start[g.n] = seqs[i].start; g.len[g.n] = seqs[i].len; g.table[g.n] = seqs[i].table; g.pos0[g.n] = seqs[i].pos0;
+        ++g.n;
+    }
     int nl = 0;
     // linear layers: wgmma / TMA GEMM (prefill_tc5.cu); GL_PREFILL_TC5=0 keeps the mma.sync kernel for A/B runs
     auto linear = [&](const GemmParams& g) -> cudaError_t {
         if (prefill_tc5_ && gemm_tc5_supported(g)) return gemm_tc5_launch(g, tp, bf, s);
         return gemm_tn_launch(g, bf, s);
     };
-    CU(embed_rows_launch(tok_embd_.w, tok_embd_.type, n_embd_, tok_embd_.row_stride, prompt_ids_ + pos0, T, pf_x_, s)); ++nl;
+    CU(embed_rows_launch(tok_embd_.w, tok_embd_.type, n_embd_, tok_embd_.row_stride, ids, t_rows, pf_x_, s)); ++nl;
     const float scale = 1.0f / std::sqrt((float)hd_);
-    PrefillSegs segs{};
-    segs.n = 1; segs.start[0] = 0; segs.len[0] = T; segs.table[0] = page_table_; segs.pos0[0] = pos0;
     for (int il = 0; il < n_layer_; ++il) {
         const LayerWeights& L = layers_[il];
-        __half* kc = kcache_ + (size_t)il * kv_layer_elems_;
-        __half* vc = vcache_ + (size_t)il * kv_layer_elems_;
-        CU(rmsnorm_rows_launch(pf_x_, L.attn_norm, T, TP, n_embd_, eps_, pf_xn_, bf, s)); ++nl;
+        __half* kc = cached ? kcache_ + (size_t)il * kv_layer_elems_ : nullptr;
+        __half* vc = cached ? vcache_ + (size_t)il * kv_layer_elems_ : nullptr;
+        CU(rmsnorm_rows_launch(pf_x_, L.attn_norm, t_rows, TP, n_embd_, eps_, pf_xn_, bf, s)); ++nl;
         bool roped = false;
         {
             GemmParams g{};
             ST(prompt_operand(L, OP_QKV, &g.b, &nl));
-            g.a = pf_xn_; g.c = pf_qkv_; g.m = T; g.n = ldq; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = ldq;
+            g.a = pf_xn_; g.c = pf_qkv_; g.m = t_rows; g.n = ldq; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = ldq;
             g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_F32;
-            RopeSplitArgs ra{rope_cos_, rope_sin_, pf_q_, pf_k_, pf_vt_, kc, vc, n_head_, n_kv_, hd_, tp, segs};
-            if (prefill_flash_ && prefill_fuse_rope_ && prefill_tc5_) {
-                // RoPE + split + cache append in the projection's own epilogue: the fp32 QKV matrix never exists (rows T .. TP of
-                // the normalised activations are zeros; the epilogue writes them as padding rows)
+            if (prefill_flash_ && prefill_fuse_rope_ && prefill_tc5_ && groups.size() == 1) {
+                // RoPE + split + cache append in the projection's own epilogue: the fp32 QKV matrix never exists (rows t_rows .. TP
+                // of the normalised activations are zeros; the epilogue writes them as padding rows)
+                RopeSplitArgs ra{rope_cos_, rope_sin_, pf_q_, pf_k_, pf_vt_, kc, vc, n_head_, n_kv_, hd_, tp, groups[0]};
                 GemmParams gr = g;
                 gr.epi = GEMM_EPI_ROPE_SPLIT; gr.rope = &ra; gr.m = TP;
                 if (gemm_tc5_supported(gr)) { CU(gemm_tc5_launch(gr, tp, bf, s)); ++nl; roped = true; }
@@ -179,47 +191,68 @@ Status Engine::prefill_chunk(int pos0, int n, int* n_launch) {
             if (!roped) { CU(linear(g)); ++nl; }
         }
         if (prefill_flash_) {
-            // (RoPE + split + cache append, then) ONE fused attention launch (prefill_attn.cu): scores stay on the SM
-            if (!roped) { CU(rope_split_segs_launch(pf_qkv_, TP, n_head_, n_kv_, hd_, rope_cos_, rope_sin_, pf_q_, pf_k_, pf_vt_, kc, vc, tp, segs, s)); ++nl; }
-            CU(flash_prefill_launch(pf_q_, pf_k_, pf_vt_, (__half*)pf_attn_, segs, n_head_, n_kv_, hd_, tp, scale, kc, vc, s));
-            ++nl;
-        } else {
-            CU(rope_split_launch(pf_qkv_, T, tp, 0, n_head_, n_kv_, hd_, rope_cos_, rope_sin_, pf_q_, pf_k_, pf_vt_, kc, vc, page_table_, tp, s)); ++nl;
-            {   // S[h] = Q_h K_kvh^T
-                GemmParams g{};
-                g.a = pf_q_; g.b = pf_k_; g.c = pf_s_; g.m = T; g.n = T; g.k = hd_; g.lda = qd; g.ldb = kvd; g.ldc = tp;
-                g.batch = n_head_; g.a_batch_stride = hd_; g.b_batch_stride = hd_; g.b_batch_div = grp; g.c_batch_stride = (long long)tp * tp;
-                g.epi = GEMM_EPI_F32; g.causal_skip = 1;
-                CU(gemm_tn_launch(g, false, s)); ++nl;
+            // (RoPE + split + cache append, then) ONE fused attention launch per segment list (prefill_attn.cu): scores stay on the SM
+            for (size_t c = 0; c < groups.size(); ++c) {
+                const PrefillSegs& segs = groups[c];
+                if (!roped) {
+                    // the kernel indexes rows of its list absolutely: shift the segment starts to the list's first row; the
+                    // trailing rows of the pass are zeroed too
+                    PrefillSegs rs = segs;
+                    const int row_lo = segs.start[0];
+                    int row_hi = c + 1 == groups.size() ? TP : row_lo;
+                    for (int i = 0; i < rs.n; ++i) {
+                        row_hi = std::max(row_hi, segs.start[i] + (segs.len[i] + 127) / 128 * 128);
+                        rs.start[i] -= row_lo;
+                    }
+                    CU(rope_split_segs_launch(pf_qkv_ + (size_t)row_lo * ldq, row_hi - row_lo, n_head_, n_kv_, hd_, rope_cos_, rope_sin_, pf_q_ + (size_t)row_lo * qd,
+                                              pf_k_ + (size_t)row_lo * kvd, pf_vt_ + row_lo, kc, vc, tp, rs, s)); ++nl;
+                }
+                CU(flash_prefill_launch(pf_q_, pf_k_, pf_vt_, (__half*)pf_attn_, segs, n_head_, n_kv_, hd_, tp, scale, kc, vc, s));
+                ++nl;
             }
-            CU(softmax_causal_launch(pf_s_, n_head_, T, tp, scale, pf_p_, s)); ++nl;
-            {   // O[:, h] = P[h] V_kvh   (B = V^T rows = head dims)
-                GemmParams g{};
-                g.a = pf_p_; g.b = pf_vt_; g.c = pf_attn_; g.m = T; g.n = hd_; g.k = TP; g.lda = tp; g.ldb = tp; g.ldc = qd;
-                g.batch = n_head_; g.a_batch_stride = (long long)tp * tp; g.b_batch_stride = (long long)hd_ * tp; g.b_batch_div = grp; g.c_batch_stride = hd_;
-                g.epi = GEMM_EPI_T16; g.causal_k = 1;
-                CU(gemm_tn_launch(g, false, s)); ++nl;
+        } else {
+            // the three-launch A/B path, per sequence (every pos0 is 0 here)
+            for (const PromptSeq& q : seqs) {
+                const int r0 = q.start, len = q.len, lp = (len + 127) / 128 * 128;
+                // RoPE at positions 0..len-1 of THIS sequence; V^T columns r0.. of the pass-wide [kvd][tp] matrix
+                CU(rope_split_launch(pf_qkv_ + (size_t)r0 * ldq, len, lp, 0, n_head_, n_kv_, hd_, rope_cos_, rope_sin_, pf_q_ + (size_t)r0 * qd,
+                                     pf_k_ + (size_t)r0 * kvd, pf_vt_ + r0, kc, vc, q.table, tp, s)); ++nl;
+                {   // S[h] = Q_h K_kvh^T, compact [n_head][lp][lp]
+                    GemmParams g{};
+                    g.a = pf_q_ + (size_t)r0 * qd; g.b = pf_k_ + (size_t)r0 * kvd; g.c = pf_s_; g.m = len; g.n = len; g.k = hd_; g.lda = qd; g.ldb = kvd; g.ldc = lp;
+                    g.batch = n_head_; g.a_batch_stride = hd_; g.b_batch_stride = hd_; g.b_batch_div = grp; g.c_batch_stride = (long long)lp * lp;
+                    g.epi = GEMM_EPI_F32; g.causal_skip = 1;
+                    CU(gemm_tn_launch(g, false, s)); ++nl;
+                }
+                CU(softmax_causal_launch(pf_s_, n_head_, len, lp, scale, pf_p_, s)); ++nl;
+                {   // O[:, h] = P[h] V_kvh   (B = V^T rows = head dims)
+                    GemmParams g{};
+                    g.a = pf_p_; g.b = pf_vt_ + r0; g.c = (__half*)pf_attn_ + (size_t)r0 * qd; g.m = len; g.n = hd_; g.k = lp; g.lda = lp; g.ldb = tp; g.ldc = qd;
+                    g.batch = n_head_; g.a_batch_stride = (long long)lp * lp; g.b_batch_stride = (long long)hd_ * tp; g.b_batch_div = grp; g.c_batch_stride = hd_;
+                    g.epi = GEMM_EPI_T16; g.causal_k = 1;
+                    CU(gemm_tn_launch(g, false, s)); ++nl;
+                }
             }
         }
         {
             GemmParams g{};
             ST(prompt_operand(L, OP_O, &g.b, &nl));
-            g.a = pf_attn_; g.c = pf_x_; g.m = T; g.n = n_embd_; g.k = qd; g.lda = qd; g.ldb = qd; g.ldc = n_embd_;
+            g.a = pf_attn_; g.c = pf_x_; g.m = t_rows; g.n = n_embd_; g.k = qd; g.lda = qd; g.ldb = qd; g.ldc = n_embd_;
             g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_ADD_F32;
             CU(linear(g)); ++nl;
         }
-        CU(rmsnorm_rows_launch(pf_x_, L.ffn_norm, T, TP, n_embd_, eps_, pf_xn_, bf, s)); ++nl;
+        CU(rmsnorm_rows_launch(pf_x_, L.ffn_norm, t_rows, TP, n_embd_, eps_, pf_xn_, bf, s)); ++nl;
         {
             GemmParams g{};
             ST(prompt_operand(L, OP_GU, &g.b, &nl));
-            g.a = pf_xn_; g.c = pf_h_; g.m = T; g.n = 2 * n_ff_; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = n_ff_;
+            g.a = pf_xn_; g.c = pf_h_; g.m = t_rows; g.n = 2 * n_ff_; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = n_ff_;
             g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_SILU;
             CU(linear(g)); ++nl;
         }
         {
             GemmParams g{};
             ST(prompt_operand(L, OP_DOWN, &g.b, &nl));
-            g.a = pf_h_; g.c = pf_x_; g.m = T; g.n = n_embd_; g.k = n_ff_; g.lda = n_ff_; g.ldb = n_ff_; g.ldc = n_embd_;
+            g.a = pf_h_; g.c = pf_x_; g.m = t_rows; g.n = n_embd_; g.k = n_ff_; g.lda = n_ff_; g.ldb = n_ff_; g.ldc = n_embd_;
             g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_ADD_F32;
             CU(linear(g)); ++nl;
         }
@@ -228,125 +261,16 @@ Status Engine::prefill_chunk(int pos0, int n, int* n_launch) {
     return {};
 }
 
-// Packed prompt pass for embeddings (generateEmbedding with `input: string[]`, /root/reference/server/src/routes/ollama.ts:574-643 ->
-// client/src/services/OllamaService.ts:619-636): the sequences of a call share the linear layers -- one [T x n_embd] activation
-// matrix, T = all their tokens, every weight matrix read once per PACK instead of once per sequence -- and attend only inside
-// themselves (block-diagonal causal attention: the three attention launches run per sequence on its own rows).  Nothing is
-// cached: an embedding has no decode phase.  Hidden states end up in pf_x_ for pooling.
-Status Engine::prefill_packed(const std::vector<int>& starts, const std::vector<int>& lens, int t_rows, int* n_launch,
-                              const std::vector<const int*>* tables, const std::vector<int>* pos0) {
-    if (pos0 && !prefill_flash_)
-        for (int p : *pos0)
-            if (p > 0) return failp(GL_ERR_UNSUPPORTED, "a prompt pass from a non-zero position needs the fused prompt attention");
-    const int TP = (t_rows + 127) / 128 * 128;
-    const int qd = n_head_ * hd_, kvd = n_kv_ * hd_, ldq = qd + 2 * kvd, grp = n_head_ / n_kv_;
-    ST(ensure_prefill_scratch(std::max(TP, 128)));
-    const int tp = pf_cap_;
-    cudaStream_t s = stream_;
-    const bool bf = prefill_bf16_;
-    int nl = 0;
-    auto linear = [&](const GemmParams& g) -> cudaError_t {
-        if (prefill_tc5_ && gemm_tc5_supported(g)) return gemm_tc5_launch(g, tp, bf, s);
-        return gemm_tn_launch(g, bf, s);
+Status Engine::ensure_pack_buffers() {
+    if (pk_ids_) return {};
+    auto dalloc = [&](void** p, size_t bytes) -> cudaError_t {
+        cudaError_t e = cudaMalloc(p, bytes);
+        if (e == cudaSuccess) allocs_.push_back(*p);
+        return e;
     };
-    CU(embed_rows_launch(tok_embd_.w, tok_embd_.type, n_embd_, tok_embd_.row_stride, pk_ids_, TP, pf_x_, s)); ++nl;
-    const float scale = 1.0f / std::sqrt((float)hd_);
-    for (int il = 0; il < n_layer_; ++il) {
-        const LayerWeights& L = layers_[il];
-        __half* kc = tables ? kcache_ + (size_t)il * kv_layer_elems_ : nullptr;      // gl_seq_open_many: each sequence's K / V rows go
-        __half* vc = tables ? vcache_ + (size_t)il * kv_layer_elems_ : nullptr;      // to its own pages; embeddings cache nothing
-        CU(rmsnorm_rows_launch(pf_x_, L.attn_norm, TP, TP, n_embd_, eps_, pf_xn_, bf, s)); ++nl;
-        bool roped = false;
-        {
-            GemmParams g{};
-            ST(prompt_operand(L, OP_QKV, &g.b, &nl));
-            g.a = pf_xn_; g.c = pf_qkv_; g.m = TP; g.n = ldq; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = ldq;
-            g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_F32;
-            RopeSplitArgs ra{rope_cos_, rope_sin_, pf_q_, pf_k_, pf_vt_, kc, vc, n_head_, n_kv_, hd_, tp, {}};
-            if (prefill_flash_ && prefill_fuse_rope_ && prefill_tc5_ && starts.size() <= (size_t)PF_MAX_SEGS) {
-                ra.segs.n = (int)starts.size();
-                for (int i = 0; i < ra.segs.n; ++i) {
-                    ra.segs.start[i] = starts[i];
-                    ra.segs.len[i] = lens[i];
-                    ra.segs.table[i] = tables ? (*tables)[i] : nullptr;
-                    ra.segs.pos0[i] = pos0 ? (*pos0)[i] : 0;
-                }
-                GemmParams gr = g;
-                gr.epi = GEMM_EPI_ROPE_SPLIT; gr.rope = &ra;
-                if (gemm_tc5_supported(gr)) { CU(gemm_tc5_launch(gr, tp, bf, s)); ++nl; roped = true; }
-            }
-            if (!roped) { CU(linear(g)); ++nl; }
-        }
-        if (prefill_flash_) {
-            // the whole pack: one RoPE / split launch and one fused attention launch per PF_MAX_SEGS sequences
-            for (size_t c0 = 0; c0 < starts.size(); c0 += PF_MAX_SEGS) {
-                PrefillSegs segs{};
-                segs.n = (int)std::min<size_t>(PF_MAX_SEGS, starts.size() - c0);
-                int row_lo = starts[c0], row_hi = row_lo;
-                for (int i = 0; i < segs.n; ++i) {
-                    segs.start[i] = starts[c0 + i];
-                    segs.len[i] = lens[c0 + i];
-                    segs.table[i] = tables ? (*tables)[c0 + i] : nullptr;
-                    segs.pos0[i] = pos0 ? (*pos0)[c0 + i] : 0;
-                    row_hi = std::max(row_hi, segs.start[i] + (segs.len[i] + 127) / 128 * 128);
-                }
-                if (c0 + PF_MAX_SEGS >= starts.size()) row_hi = std::max(row_hi, TP);      // trailing rows of the pack are zeroed too
-                // the kernel indexes rows of the pack absolutely: shift the segment starts to the chunk's first row
-                if (!roped) {
-                    PrefillSegs rs = segs;
-                    for (int i = 0; i < rs.n; ++i) rs.start[i] -= row_lo;
-                    CU(rope_split_segs_launch(pf_qkv_ + (size_t)row_lo * ldq, row_hi - row_lo, n_head_, n_kv_, hd_, rope_cos_, rope_sin_, pf_q_ + (size_t)row_lo * qd,
-                                              pf_k_ + (size_t)row_lo * kvd, pf_vt_ + row_lo, kc, vc, tp, rs, s)); ++nl;
-                }
-                CU(flash_prefill_launch(pf_q_, pf_k_, pf_vt_, (__half*)pf_attn_, segs, n_head_, n_kv_, hd_, tp, scale, kc, vc, s));
-                ++nl;
-            }
-        } else
-        for (size_t i = 0; i < starts.size(); ++i) {
-            const int r0 = starts[i], len = lens[i], lp = (len + 127) / 128 * 128;
-            // RoPE at positions 0..len-1 of THIS sequence; V^T columns r0.. of the pack-wide [kvd][tp] matrix; no cache
-            CU(rope_split_launch(pf_qkv_ + (size_t)r0 * ldq, len, lp, 0, n_head_, n_kv_, hd_, rope_cos_, rope_sin_, pf_q_ + (size_t)r0 * qd,
-                                 pf_k_ + (size_t)r0 * kvd, pf_vt_ + r0, kc, vc, tables ? (*tables)[i] : nullptr, tp, s)); ++nl;
-            {   // S[h] = Q_h K_kvh^T, compact [n_head][lp][lp]
-                GemmParams g{};
-                g.a = pf_q_ + (size_t)r0 * qd; g.b = pf_k_ + (size_t)r0 * kvd; g.c = pf_s_; g.m = len; g.n = len; g.k = hd_; g.lda = qd; g.ldb = kvd; g.ldc = lp;
-                g.batch = n_head_; g.a_batch_stride = hd_; g.b_batch_stride = hd_; g.b_batch_div = grp; g.c_batch_stride = (long long)lp * lp;
-                g.epi = GEMM_EPI_F32; g.causal_skip = 1;
-                CU(gemm_tn_launch(g, false, s)); ++nl;
-            }
-            CU(softmax_causal_launch(pf_s_, n_head_, len, lp, scale, pf_p_, s)); ++nl;
-            {   // O[:, h] = P[h] V_kvh
-                GemmParams g{};
-                g.a = pf_p_; g.b = pf_vt_ + r0; g.c = (__half*)pf_attn_ + (size_t)r0 * qd; g.m = len; g.n = hd_; g.k = lp; g.lda = lp; g.ldb = tp; g.ldc = qd;
-                g.batch = n_head_; g.a_batch_stride = (long long)lp * lp; g.b_batch_stride = (long long)hd_ * tp; g.b_batch_div = grp; g.c_batch_stride = hd_;
-                g.epi = GEMM_EPI_T16; g.causal_k = 1;
-                CU(gemm_tn_launch(g, false, s)); ++nl;
-            }
-        }
-        {
-            GemmParams g{};
-            ST(prompt_operand(L, OP_O, &g.b, &nl));
-            g.a = pf_attn_; g.c = pf_x_; g.m = TP; g.n = n_embd_; g.k = qd; g.lda = qd; g.ldb = qd; g.ldc = n_embd_;
-            g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_ADD_F32;
-            CU(linear(g)); ++nl;
-        }
-        CU(rmsnorm_rows_launch(pf_x_, L.ffn_norm, TP, TP, n_embd_, eps_, pf_xn_, bf, s)); ++nl;
-        {
-            GemmParams g{};
-            ST(prompt_operand(L, OP_GU, &g.b, &nl));
-            g.a = pf_xn_; g.c = pf_h_; g.m = TP; g.n = 2 * n_ff_; g.k = n_embd_; g.lda = n_embd_; g.ldb = n_embd_; g.ldc = n_ff_;
-            g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_SILU;
-            CU(linear(g)); ++nl;
-        }
-        {
-            GemmParams g{};
-            ST(prompt_operand(L, OP_DOWN, &g.b, &nl));
-            g.a = pf_h_; g.c = pf_x_; g.m = TP; g.n = n_embd_; g.k = n_ff_; g.lda = n_ff_; g.ldb = n_ff_; g.ldc = n_embd_;
-            g.batch = 1; g.b_batch_div = 1; g.epi = GEMM_EPI_ADD_F32;
-            CU(linear(g)); ++nl;
-        }
-    }
-    if (n_launch) *n_launch += nl;
+    CU(dalloc((void**)&pk_ids_, (size_t)EMB_PACK_TOKENS * 4));
+    CU(dalloc((void**)&emb_pooled_, (size_t)n_embd_ * 4));
+    CU(dalloc((void**)&emb_rstd_, (size_t)std::max(EMB_PACK_TOKENS, n_ctx_) * 4));
     return {};
 }
 
